@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""bench.py -- compress+decompress throughput of the block-sorting hot path on B200.
+"""bench.py -- compress+decompress throughput of the block-sorting hot path on an H100.
 
 One "step" = one pass of the hot path over this rank's batch of synthetic blocks: every block is
 compressed (adler32 -> forward BWT -> QLFC static coder -> framing) and then decompressed (QLFC
@@ -18,8 +18,11 @@ context / stream, so the HBM-bound sorts of some blocks overlap the latency-boun
           (oracle/ref_driver.c) on the box's host cores.
 
 Workload (BASELINE.json config C3, per GPU): G_text(seed 2 + rank), 64 blocks of 64 MiB per step, sorter BWT,
-coder QLFC static, LZP off.  64 blocks = 512 coder streams for the 296 coder slots of a B200 (two CTAs per SM).
+coder QLFC static, LZP off.  64 blocks = 512 coder streams, more than the encoder slots of an H100 (two to four CTAs per SM on 132 SMs).
 Weak scaling: every rank processes its own 4 GiB per step.
+
+--dump-outputs DIR writes what the timed steps' last step returned to its caller (see dump_outputs), so that two builds can be
+compared output for output on identical seeded inputs.
 """
 import argparse
 import ctypes
@@ -51,7 +54,7 @@ def parse_args():
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--blocks", type=int, default=64, help="blocks per GPU and step")
     ap.add_argument("--block-mib", type=int, default=64)
-    ap.add_argument("--workers", type=int, default=0, help="blocks in flight per GPU = contexts = worker threads (0 = 96, or all blocks of a step of fewer than 64 blocks)")
+    ap.add_argument("--workers", type=int, default=0, help="blocks in flight per GPU = contexts = worker threads (0 = as many as the free HBM holds, at most 96 and at most the blocks of a step)")
     ap.add_argument("--sorter", type=int, default=1)
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--ref-blocks", type=int, default=16, help="blocks per step of the reference arm / cpu_baseline leg (see reference_sample_blocks)")
@@ -59,18 +62,28 @@ def parse_args():
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--e2e-steps", type=int, default=12, help="the end-to-end (host buffer) leg times min(--steps, this) steps, so that a long --steps run still ends within minutes")
     ap.add_argument("--no-extras", dest="extras", action="store_false", help="skip the extra keys for BASELINE configs C2 / C3-strong / C4 / C5")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the outputs of the last timed step to DIR/<name>.npy")
+    args = ap.parse_args()
+    if args.steps < 1 or args.warmup < 0:
+        ap.error("--steps must be >= 1 and --warmup >= 0")
+    return args
 
 
 # ------------------------------------------------------------------------------------------------
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region, and the card's name and power limit (part of every number)."""
     Q = "index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
 
     def __init__(self, index):
-        self.index, self.proc, self.lines = index, None, []
+        self.index, self.proc, self.lines, self.card = index, None, [], {}
 
     def start(self):
+        try:
+            f = subprocess.run(["nvidia-smi", "-i", str(self.index), "--query-gpu=name,power.limit", "--format=csv,noheader,nounits"],
+                               capture_output=True, text=True, timeout=30).stdout.strip().split(",")
+            self.card = {"gpu": f[0].strip(), "power_limit_w": float(f[1])} if len(f) == 2 else {}
+        except Exception:
+            pass
         try:
             self.proc = subprocess.Popen(["nvidia-smi", "-i", str(self.index), "--query-gpu=" + self.Q, "--format=csv,noheader,nounits", "-lms", "200"],
                                          stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True)
@@ -85,6 +98,7 @@ class ClockSampler:
     def stop(self):
         if self.proc:
             self.proc.terminate()
+            self.proc.wait()
         sm, mx, reasons = [], 0, set()
         for ln in self.lines:
             f = [x.strip() for x in ln.split(",")]
@@ -97,7 +111,7 @@ class ClockSampler:
             for name, v in zip(("hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"), f[4:8]):
                 if v.lower().startswith("active"):
                     reasons.add(name)
-        return {"sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": mx or None, "reasons": sorted(reasons), "samples": len(sm)}
+        return dict(self.card, sm_mhz=float(np.median(sm)) if sm else None, sm_max_mhz=mx or None, reasons=sorted(reasons), samples=len(sm))
 
 
 def make_blocks(gen, seed, nblocks, block_bytes):
@@ -129,10 +143,8 @@ def run_reference(args, rank, world):
 
 def reference_sample_blocks(args, world=1):
     """Blocks per step of the reference arm: a BOUNDED sample of the GPU arm's workload (same generator, block size, sorter, coder).
-    16 blocks of 64 MiB = BASELINE C3's 1 GiB, one block per OpenMP thread as the reference CLI does (bsc.cpp:184-199).  Measured on the
-    B200 box's host (128 hardware threads): 16 blocks / 16 threads 145.6 MB/s, 18 / 18 144-159 MB/s, 64 / 64 109-117 MB/s at 39 s per step
-    (profiles/r1g, r1h, r2i) -- more blocks at once make the reference SLOWER (memory-bound suffix sorting), so the sample is also its
-    best configuration, and a --steps 20 --warmup 5 run ends in ~3.5 minutes instead of 16."""
+    16 blocks of 64 MiB = BASELINE C3's 1 GiB, one block per OpenMP thread as the reference CLI does (bsc.cpp:184-199).  More blocks at
+    once do not make the memory-bound suffix sorting of the reference faster, and the bounded sample keeps the leg to minutes."""
     threads = len(os.sched_getaffinity(0))
     return max(1, min(world * args.blocks, threads, args.ref_blocks))
 
@@ -221,10 +233,34 @@ def reference_stage_seconds(args):
 def workload_config(args, extra=None):
     c = {"workload": "C3: G_text(seed 2+rank) %d x %d MiB blocks per GPU, BWT + QLFC static, LZP off (-b%d -m0 -e1 -p)" % (args.blocks, args.block_mib, args.block_mib),
          "blocks_per_gpu": args.blocks, "block_bytes": args.block_mib << 20, "sorter": args.sorter, "coder": 1,
-         "l2": "inputs_larger_than_L2 (%d MiB per step vs 126 MB L2)" % (args.blocks * args.block_mib)}
+         "l2": "inputs_larger_than_L2 (%d MiB per step vs 50 MB L2)" % (args.blocks * args.block_mib)}
     if extra:
         c.update(extra)
     return c
+
+
+def dump_outputs(out_dir, prefix, d_cmp, csize, d_back, bb, sample_bytes):
+    """The arrays the last timed step handed back for every block: its compressed block (the bytes after the 4-byte alignment pad of the
+    device buffer) and its restored bytes.  Whole outputs are pinned by their size and Adler-32; their bytes by a fixed, seeded sample of
+    positions, the two float32 sample arrays together at most `sample_bytes`.  Float64 / float32 .npy files."""
+    import zlib
+    nb = len(d_cmp)
+    k = max(1, min(65536, sample_bytes // (2 * 4 * nb)))
+    rng = np.random.default_rng(20240601)
+    pos_back = np.sort(rng.integers(0, bb, k))
+    c_adler, c_sample, b_adler, b_sample = [], [], [], []
+    for i in range(nb):
+        c = d_cmp[i][4:4 + csize[i]].cpu().numpy()
+        c_adler.append(zlib.adler32(c.tobytes()))
+        c_sample.append(c[np.sort(rng.integers(0, c.size, k))])
+        b = d_back[i][:bb].cpu().numpy()
+        b_adler.append(zlib.adler32(b.tobytes()))
+        b_sample.append(b[pos_back])
+    os.makedirs(out_dir, exist_ok=True)
+    for name, arr in (("compressed_sizes", np.array(csize, np.float64)), ("compressed_adler32", np.array(c_adler, np.float64)),
+                      ("compressed_sample", np.array(c_sample, np.float32)), ("restored_adler32", np.array(b_adler, np.float64)),
+                      ("restored_sample", np.array(b_sample, np.float32))):
+        np.save(os.path.join(out_dir, prefix + name + ".npy"), arr)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -234,8 +270,9 @@ class Pipeline:
     sorts of some overlap the latency-bound coder kernels of others, and the SM slots a short coder stream frees are taken by the
     next block's streams.  W (blocks in flight) is independent of the number of blocks per step."""
 
-    def __init__(self, nb, workers, task, block_buffers=False):
+    def __init__(self, nb, workers, task, block_buffers=False, last_task=None):
         self.nb, self.workers, self.task = nb, workers, task
+        self.last_task = last_task or task                          # runs the tasks of the last step of every run()
         # block_buffers: the task writes per-BLOCK buffers (extra_configs), so a block belongs to one task at a time (step s+1 may catch up with step s)
         self.block_lock = [threading.Lock() for _ in range(nb)] if block_buffers else None
 
@@ -250,11 +287,12 @@ class Pipeline:
                         t = nxt[0]; nxt[0] += 1
                     if t >= total or errs:
                         return
+                    task = self.last_task if t >= total - self.nb else self.task
                     if self.block_lock:
                         with self.block_lock[t % self.nb]:
-                            self.task(w, t % self.nb)
+                            task(w, t % self.nb)
                     else:
-                        self.task(w, t % self.nb)
+                        task(w, t % self.nb)
             except BaseException as ex:                              # surface the first failure, stop the others
                 errs.append(ex)
         ths = [threading.Thread(target=loop, args=(w,)) for w in range(min(self.workers, total))]
@@ -376,19 +414,23 @@ def run_b200(args, rank, local_rank, world):
     gen = pyoracle.Gen()
     nb, bb = args.blocks, args.block_mib << 20
     host_blocks = make_blocks(gen, 2 + rank, nb, bb)
-    # blocks in flight = contexts = worker threads, independent of the blocks per step.  96 keep the 740 decoder slots of a B200 (five per SM)
-    # and six sort slabs busy (A/B: 64 / 96 / 128 in flight -> 768 / 836 / 815 MB/s, profiles/r2i_call_i.log, r2j_call_j.log)
-    workers = args.workers if args.workers > 0 else (96 if nb >= 64 else nb)
 
     # ---- device-resident leg ------------------------------------------------------------------
     # inputs per block; compressed / restored buffers per WORKER (a task = compress block i, then decompress it, on one context),
     # plus one compressed buffer per block for the passes that run each direction alone
     d_in = [torch.from_numpy(b).to(dev) for b in host_blocks]
+    d_cmp_blk = [torch.empty(bb + 28 + 64, dtype=torch.uint8, device=dev) for _ in range(nb)]
+    # --dump-outputs: the last timed step restores every block into a buffer of its own, kept for dump_outputs
+    d_back_blk = [torch.empty(bb + 64, dtype=torch.uint8, device=dev) for _ in range(nb)] if args.dump_outputs else None
+    ws = int(L.bscb200_workspace_bytes(bb, args.sorter))
+    # blocks in flight = contexts = worker threads, independent of the blocks per step.  Up to 96 (enough to keep five decoder streams per
+    # SM busy at eight streams per block), as many as the free HBM holds beside the library's six shared sort slabs and 5 % headroom
+    per_worker = ws + 2 * (bb + 128)
+    room = int(L.bscb200_device_free_bytes()) - 6 * int(L.bscb200_scratch_bytes(bb, args.sorter))
+    workers = args.workers if args.workers > 0 else max(1, min(96 if nb >= 64 else nb, int(room * 0.95) // per_worker))
     d_cmp = [torch.empty(bb + 28 + 64, dtype=torch.uint8, device=dev) for _ in range(workers)]
     d_back = [torch.empty(bb + 64, dtype=torch.uint8, device=dev) for _ in range(workers)]
-    d_cmp_blk = [torch.empty(bb + 28 + 64, dtype=torch.uint8, device=dev) for _ in range(nb)]
     ctxs = [libbsc_b200.DeviceCtx(local_rank) for _ in range(workers)]
-    ws = int(L.bscb200_workspace_bytes(bb, args.sorter))
     for c in ctxs:
         assert c.reserve(ws) == 0, "workspace allocation failed"
     csize = [0] * nb
@@ -400,14 +442,22 @@ def run_b200(args, rank, local_rank, world):
         assert r > 0, "compress failed: %d" % r
         csize[i] = r
 
-    def dev_decompress(w, i, src=None):
-        r = ctxs[w].decompress((d_cmp[w] if src is None else src).data_ptr() + 4, csize[i], d_back[w].data_ptr(), bb, 3)
+    def dev_decompress(w, i, src=None, dst=None):
+        r = ctxs[w].decompress((d_cmp[w] if src is None else src).data_ptr() + 4, csize[i], (d_back[w] if dst is None else dst).data_ptr(), bb, 3)
         assert r == 0, "decompress failed: %d" % r
-        last[w] = i
+        if dst is None:
+            last[w] = i
 
     def dev_task(w, i):
         torch.cuda.set_device(local_rank)
         dev_compress(w, i); dev_decompress(w, i)
+
+    def dev_task_kept(w, i):                             # the same work, results left in the block's own buffers (--dump-outputs)
+        torch.cuda.set_device(local_rank)
+        dev_compress(w, i, d_cmp_blk[i]); dev_decompress(w, i, d_cmp_blk[i], d_back_blk[i])
+
+    def dev_decompress_kept(w, i):
+        dev_decompress(w, i, d_cmp_blk[i], d_back_blk[i])
 
     def dev_compress_blk(w, i):
         dev_compress(w, i, d_cmp_blk[i])
@@ -441,18 +491,21 @@ def run_b200(args, rank, local_rank, world):
     class Steps:
         """--mode pipeline: compress -> decompress per block, all blocks and steps as one flow.  --mode phased: per step every block is
         compressed, then every block is decompressed (the sorts of the compress phase find the SMs free of coder CTAs)."""
-        def __init__(self, task, comp, decomp):
-            self.flow, self.comp, self.decomp = Pipeline(nb, workers, task), Pipeline(nb, workers, phase(comp)), Pipeline(nb, workers, phase(decomp))
+        def __init__(self, task, comp, decomp, task_kept=None, decomp_kept=None):
+            self.flow, self.comp, self.decomp = Pipeline(nb, workers, task, last_task=task_kept), Pipeline(nb, workers, phase(comp)), Pipeline(nb, workers, phase(decomp))
+            self.decomp_last = Pipeline(nb, workers, phase(decomp_kept or decomp))
 
         def run(self, steps):
             if args.mode == "pipeline":
                 self.flow.run(steps)
             else:
-                for _ in range(steps):
-                    self.comp.run(1); self.decomp.run(1)
+                for s in range(steps):
+                    self.comp.run(1); (self.decomp_last if s == steps - 1 else self.decomp).run(1)
 
     pipe = Steps(dev_task, dev_compress_blk, dev_decompress_blk)
     pipe.run(args.warmup)
+    if args.dump_outputs:
+        pipe = Steps(dev_task, dev_compress_blk, dev_decompress_blk, dev_task_kept, dev_decompress_kept)
     for c in ctxs:
         c.set_profile(True)
     launches0 = sum(c.launches() for c in ctxs)
@@ -464,6 +517,12 @@ def run_b200(args, rank, local_rank, world):
     launches = sum(c.launches() for c in ctxs) - launches0
     for w in range(workers):                             # what the timed steps left behind: each worker's last block
         assert last[w] < 0 or torch.equal(d_back[w][:bb], d_in[last[w]]), "round trip mismatch in block %d" % last[w]
+    if args.dump_outputs:
+        for i in range(nb):                              # the blocks of the last step were restored into buffers of their own
+            assert torch.equal(d_back_blk[i][:bb], d_in[i]), "round trip mismatch in block %d" % i
+        # 60 * 10^6 bytes of samples over all ranks: with the sizes and checksums the files stay within 64 MB in all
+        dump_outputs(args.dump_outputs, "" if world == 1 else "rank%d_" % rank, d_cmp_blk, csize, d_back_blk, bb, 60 * 10**6 // world)
+        del d_back_blk
     # per-kernel CUDA-event timings gathered during the timed steps
     kern = {}
     for c in ctxs:
@@ -562,13 +621,11 @@ def run_b200(args, rank, local_rank, world):
         return
 
     # ---- roofline of the dominant kernel + per-kernel table ------------------------------------
-    peaks = {}
-    try:
-        peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-    except Exception:
-        pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
-    peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "fallback 6650 GB/s (B200_PROFILING.md)"
+    # HBM GB/s of NVIDIA's data sheets, by the name the card reports (the SXM card reports "H100 80GB HBM3"): a bound, never a measurement
+    card = torch.cuda.get_device_name(dev)
+    peak, model = next(((v, m) for m, v in (("H100 NVL", 3900.0), ("H100 PCIe", 2000.0), ("H100", 3350.0)) if m in card), (3350.0, None))
+    peak_src = ("%s data sheet, %.0f GB/s" % (model if model != "H100" else "H100 SXM", peak)) if model else \
+               "%s is not an H100: the H100 SXM data sheet's 3350 GB/s is used, the fractions do not describe this card" % card
     tot_ms = sum(v[1] for v in kern.values()) or 1.0
     table = []
     for name, (cnt, ms, by) in sorted(kern.items(), key=lambda kv: -kv[1][1]):
@@ -576,38 +633,17 @@ def run_b200(args, rank, local_rank, world):
         if by > 0:
             row["algorithmic_GBps"] = round(by / 1e9 / (ms / 1e3), 2); row["frac_of_peak"] = round(by / 1e9 / (ms / 1e3) / peak, 5)
         table.append(row)
-    prof = {}
-    try:
-        prof = json.load(open(os.path.join(ROOT, "profiles", "roofline_traffic.json")))
-    except Exception:
-        pass
     dom = table[0] if table else {"kernel": None}
     dom_bytes = kern[dom["kernel"]][2] if table else 0
     dom_ms = kern[dom["kernel"]][1] if table else 1
     dom_cnt = kern[dom["kernel"]][0] if table else 1
     achieved = dom_bytes / 1e9 / (dom_ms / 1e3) if dom_bytes else 0.0
     roofline = {"kernel": dom["kernel"], "bound": "hbm", "achieved": round(achieved, 3), "peak": peak, "unit": "GB/s", "frac": round(achieved / peak, 6),
-                "traffic": (prof.get("dram_bytes_per_launch") or {}).get(dom["kernel"]), "peak_source": peak_src,
+                "peak_source": peak_src,
                 "bytes_per_launch": dom_bytes / max(dom_cnt, 1), "avg_launch_ms": dom_ms / max(dom_cnt, 1), "share_of_kernel_time": dom.get("share"),
                 "note": "the dominant kernel is a serial recurrence per stream (<= 8 streams per block by the format): it is bound by what one warp can "
-                        "issue, not by HBM -- see roofline_issue; launch durations of concurrent streams overlap, shares are of summed kernel time"}
-    # the bound that does apply to the coder kernels: issue slots (ncu capture committed under profiles/, keyed by kernel)
-    roofline_issue = (prof.get("issue") or {}).get(dom["kernel"])
-    try:
-        # live cross-check of the committed ncu figure: the kernel's instruction count is a property of the stream bytes (ncu, same block
-        # generator and size), its duration alone on the GPU is measured here with CUDA events -> warp instructions per cycle, summed over
-        # the streams of a launch and per stream (a LOWER bound of the per-scheduler rate: the streams of a launch end at different times)
-        if roofline_issue and dom["kernel"] in alone and clocks.get("sm_mhz") and bb == (64 << 20) and args.sorter == 1:
-            cnt_a, ms_a, _ = alone[dom["kernel"]]
-            cyc = (ms_a / max(cnt_a, 1)) * 1e-3 * clocks["sm_mhz"] * 1e6
-            per_launch = roofline_issue["instructions_per_launch"] / cyc
-            roofline_issue = dict(roofline_issue, live={"launch_ms_alone": ms_a / max(cnt_a, 1), "sm_mhz": clocks["sm_mhz"],
-                                                         "warp_instructions_per_cycle_per_launch": round(per_launch, 3),
-                                                         "per_stream_lower_bound": round(per_launch / roofline_issue.get("streams_per_launch", 8), 3)})
-    except Exception:
-        pass
-
-    # HBM-bound kernels, timed alone: achieved algorithmic GB/s against the measured copy peak
+                        "issue, not by HBM; launch durations of concurrent streams overlap, shares are of summed kernel time"}
+    # HBM-bound kernels, timed alone: achieved algorithmic GB/s against the data-sheet HBM bandwidth
     alone_table = []
     for name, (cnt, ms, by) in sorted(alone.items(), key=lambda kv: -kv[1][1]):
         row = {"kernel": name, "launches": cnt, "ms_total": round(ms, 3)}
@@ -619,7 +655,7 @@ def run_b200(args, rank, local_rank, world):
     if hbm_rows:
         r0 = hbm_rows[0]; cnt0, ms0, by0 = alone[r0["kernel"]]
         roofline_hbm = {"kernel": r0["kernel"], "bound": "hbm", "achieved": r0["algorithmic_GBps"], "peak": peak, "unit": "GB/s", "frac": r0["frac_of_peak"],
-                        "traffic": (prof.get("dram_bytes_per_launch") or {}).get(r0["kernel"]), "bytes_per_launch": by0 / max(cnt0, 1), "avg_launch_ms": ms0 / max(cnt0, 1),
+                        "bytes_per_launch": by0 / max(cnt0, 1), "avg_launch_ms": ms0 / max(cnt0, 1),
                         "how": "CUDA events around every launch, one block at a time on one stream (2 blocks), after the timed steps"}
 
     cpu = None
@@ -644,7 +680,7 @@ def run_b200(args, rank, local_rank, world):
                     "parallelism": "blocks round-robin over %d GPU(s), no collective" % world},
             "compress_MBps": total_mb / (ms_c / 1e3), "decompress_MBps": total_mb / (ms_d / 1e3), "phase_note": "each direction alone, one drained pass over the batch",
             "compressed_bytes_rank0": comp_bytes, "ratio": comp_bytes / float(nb * bb),
-            "e2e": e2e, "gpu_launches": int(launches), "clocks": clocks, "roofline": roofline, "roofline_issue": roofline_issue, "roofline_hbm_kernel": roofline_hbm,
+            "e2e": e2e, "gpu_launches": int(launches), "clocks": clocks, "roofline": roofline, "roofline_hbm_kernel": roofline_hbm,
             "other_configs": extras, "kernels": table, "kernels_standalone": alone_table, "cpu_baseline": cpu}
     print(json.dumps(line), flush=True)
 

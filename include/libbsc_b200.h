@@ -1,4 +1,4 @@
-/* include/libbsc_b200.h -- C ABI of the B200-native block-sorting hot path.
+/* include/libbsc_b200.h -- C ABI of the GPU (H100, sm_90a) block-sorting hot path.
  *
  * Drop-in boundary: the first group of functions has EXACTLY the names, argument meaning, buffer
  * ownership and error behaviour of the libbsc 3.3.5 entry points it replaces (reference file:line

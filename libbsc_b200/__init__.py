@@ -1,4 +1,4 @@
-"""libbsc_b200 -- B200-native block-sorting compression hot path (libbsc 3.3.5 compatible).
+"""libbsc_b200 -- GPU (H100, sm_90a) block-sorting compression hot path (libbsc 3.3.5 compatible).
 
 The product is the C-ABI shared library ``libbsc_b200/libbsc_b200.so`` (sources in ``csrc/``,
 interface in ``include/libbsc_b200.h``).  This package is only a thin ctypes binding of that ABI

@@ -1,4 +1,4 @@
-"""Build libbsc_b200/libbsc_b200.so (sm_100a only) with nvcc.  In-tree, incremental per source."""
+"""Build libbsc_b200/libbsc_b200.so (sm_90a, H100) with nvcc.  In-tree, incremental per source."""
 import os
 import subprocess
 import sys
@@ -11,7 +11,7 @@ LIB = os.path.join(HERE, "libbsc_b200.so")
 CLI = os.path.join(HERE, "bsc_b200")          # file-level front end (cli/bsc_b200.cpp), bsc1 container + multi-GPU block scheduler
 SOURCES = ["api.cu", "adler32.cu", "bwt_encode.cu", "bwt_decode.cu", "st_encode.cu", "st_decode.cu", "qlfc.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
          "-Xcompiler", "-fPIC,-O2,-Wall,-Wno-unused-function", "-ccbin", "/usr/bin/g++",
          "-Xptxas", "-v"] + os.environ.get("BSCB200_NVCC_EXTRA", "").split()      # e.g. -DQE_DIAG (diagnostic builds only)
 

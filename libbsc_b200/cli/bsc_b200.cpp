@@ -271,7 +271,7 @@ int decompress_file(const char *in_name, const char *out_name, Options opt)
 void usage()
 {
     fprintf(stdout,
-            "bsc_b200 -- libbsc-compatible block-sorting compressor on NVIDIA B200 GPUs (bsc1 container)\n\n"
+            "bsc_b200 -- libbsc-compatible block-sorting compressor on NVIDIA H100 GPUs (bsc1 container)\n\n"
             "Usage: bsc_b200 <e|d> inputfile outputfile <options>\n"
             "  -b<size>  block size in MiB, default -b25 (1..1024)\n"
             "  -m<algo>  block sorter: -m0 Burrows-Wheeler transform (default), -m3..-m8 sort transform of order n (encode only)\n"

@@ -15,7 +15,7 @@
 //                reaches another start row -- ONCE: the bytes it meets are staged in 128-byte slabs (node k = segment k's first
 //                slab; a segment longer than 128 bytes takes further nodes from an atomic counter and links them), so the
 //                pointer chase, which is sector/latency bound (one dependent 4-byte gather per output byte), is never repeated
-//                (round 1 walked twice: 1.2 + 2.3 ms per 64 MiB; the reference stages too, libcubwt.cu:2744-2906)
+//                (an earlier version walked twice; the reference stages too, libcubwt.cu:2744-2906)
 //   lr_jump      device-side pointer-jumping list ranking over the nodes (list_rank.cuh; no host round trip, cf.
 //                libcubwt.cu:3077-3086): bytes from the start of every node to the end of the walk
 //   unbwt_place  every staged byte goes to its final place (coalesced reads, contiguous reversed writes)
@@ -115,7 +115,7 @@ int stage_bwt_decode(Ctx *ctx, u8 *d_T, int n_, int index_)
     CUDA_TRY(cudaMemsetAsync(nlen, 0, (size_t)max_nodes, ctx->stream));                                  // unused nodes: empty ...
     CUDA_TRY(cudaMemsetAsync(pair, 0xff, sizeof(u64) * (size_t)max_nodes, ctx->stream));                 // ... and LR_DONE, so the ranking skips them
 
-    LAUNCH(ctx, unbwt_hist, min(ceil_div(n, 256 * 64), (u32)(B200_SMS * 8)), 256, 0, Lp, n, hist);
+    LAUNCH(ctx, unbwt_hist, min(ceil_div(n, 256 * 64), device_sms(ctx->device) * 8), 256, 0, Lp, n, hist);
     LAUNCH(ctx, unbwt_scan256, 1, 32, 0, hist);
     PROF_BYTES(ctx, 5.0 * n);
     LAUNCH(ctx, unbwt_lf<true>, tiles, LF_THREADS, 0, Lp, n, index, hist, hist + 256, lb, LF);

@@ -52,7 +52,7 @@ struct TileAgg { u32 maxhead, active, groups, pad; };
 
 // A tile of SC_TILE slots (+ one neighbour on each side) staged in shared memory with coalesced loads.
 // Each thread then works on 8 CONSECUTIVE slots (what the scans want); one pad entry per 8 keeps the
-// 64-byte lane stride off the same banks (profile r1d: the unstaged version spent 3 ms per 64 M slots).
+// 64-byte lane stride off the same banks (the unstaged version was measured to be bank-conflict bound).
 struct ScTile {
     u64 key[(SC_TILE + 2) + (SC_TILE + 2) / 8 + 1];
     u32 sa[(SC_TILE + 2) + (SC_TILE + 2) / 8 + 1];

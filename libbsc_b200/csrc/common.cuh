@@ -1,4 +1,4 @@
-// libbsc_b200/csrc/common.cuh -- shared device/host plumbing for the B200 block-sorting path.
+// libbsc_b200/csrc/common.cuh -- shared device/host plumbing for the GPU block-sorting path.
 //
 // One `Ctx` = one CUDA stream + one bump-allocated HBM arena + small pinned mailboxes.  Every
 // stage takes a Ctx and enqueues its kernels on ctx->stream; nothing here is global except the
@@ -9,6 +9,7 @@
 #include <cuda_runtime.h>
 #include <vector>
 #include <mutex>
+#include <atomic>
 #include <condition_variable>
 #include <stdint.h>
 #include <stdio.h>
@@ -40,7 +41,17 @@ typedef uint64_t u64;
 
 #define LIBBSC_HEADER_SIZE 28
 
-#define B200_SMS 148
+// SMs of `device` (132 on an H100 SXM), read once per device: grid sizes and the decoder layout scale with it
+static inline u32 device_sms(int device)
+{
+    static std::atomic<int> sms[16];
+    int v = sms[device & 15].load(std::memory_order_relaxed);
+    if (v <= 0) {
+        if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, device) != cudaSuccess || v <= 0) { cudaGetLastError(); v = 132; }
+        sms[device & 15].store(v, std::memory_order_relaxed);
+    }
+    return (u32)v;
+}
 
 struct CudaFail { cudaError_t err; const char *file; int line; };
 
@@ -116,7 +127,7 @@ struct Ctx {
     // Host wait for this context's stream.  cudaStreamSynchronize spins (cudaDeviceScheduleAuto), and in a full pipeline the sort kernels a
     // thread waits for are queued behind other blocks' coder CTAs for tens of milliseconds: dozens of threads per GPU (x 8 ranks per host)
     // would burn a core each.  So the wait BLOCKS on an event created with cudaEventBlockingSync (the thread sleeps until the driver's
-    // interrupt; ~30 us later than a spin would see it, ~1 ms per block).  BSCB200_SYNC=spin restores the spinning wait (A/B).
+    // interrupt, a little later than a spin would see it).  BSCB200_SYNC=spin restores the spinning wait (A/B).
     cudaEvent_t ev_sync = nullptr;
     void sync() {
         static const bool spin = [] { const char *e = getenv("BSCB200_SYNC"); return e && e[0] == 's'; }();
@@ -128,16 +139,15 @@ struct Ctx {
     // Wait for a kernel that runs for 0.01 - 2 s (the coder kernels) WITHOUT putting anything behind it on the stream and without
     // driver calls.  A process has at most 32 hardware work queues per GPU (CUDA_DEVICE_MAX_CONNECTIONS), so with 40+ blocks in
     // flight two streams share a queue; an event record or a copy enqueued behind the 2 s kernel of one of them holds the queue's head
-    // until that kernel ENDS and the other stream's work waits behind it -- measured: 48 and 64 blocks in flight ran as waves of 32
-    // (profiles/r2c_call_c.log).  Polling cudaStreamQuery from 48 threads instead made the launch-heavy sort stages of the other
-    // blocks four times slower (driver lock; profiles/r2d_call_d.log).  So the kernel itself reports: its last CTA writes a sequence
+    // until that kernel ENDS and the other stream's work waits behind it, so blocks in flight run as waves of 32.  Polling
+    // cudaStreamQuery from dozens of threads instead slows the launch-heavy sort stages of the other blocks (driver lock).  So the
+    // kernel itself reports: its last CTA writes a sequence
     // number into this context's pinned mailbox (signal_done below) and the host thread sleeps on that word.
     // Stream priorities (BSCB200_PRIO=0 turns them off).  When SM slots free up, the CTA scheduler places pending CTAs of higher-priority
     // streams first, whichever block launched first.  Three levels per context:
     //   stream     (highest)  everything that is short: the sort / scan / rank kernels.  A coder CTA holds its slot for 0.1 - 4 s, a sort
-    //                         CTA for microseconds; at equal priority the sort launches of a full pipeline ran 12 - 15 times longer than
-    //                         alone (rs_onesweep 3.8 - 5.2 ms against 0.33 ms per launch, profiles/r2i, r2j), each block spent ~2 s of its
-    //                         7.7 s round trip in sort stages and the coder slots stood half empty meanwhile;
+    //                         CTA for microseconds; at equal priority the sort launches of a full pipeline wait behind coder CTAs
+    //                         for many times their own duration while the coder slots of their blocks stand empty;
     //   stream_hi  (middle)   the LONG streams of a coder launch (qlfc.cu: split launches): longest-stream-first ACROSS blocks without any
     //                         coordination between the host threads;
     //   stream_lo  (lowest)   the other coder streams.
@@ -196,7 +206,7 @@ struct Ctx {
 
 // Optional cap on the coder CTAs in flight per device (BSCB200_CODER_SLOTS, default: none).  A coder CTA pins half an SM's shared memory for
 // 0.1 - 2 s; the sort kernels of other blocks need shared memory too and can only run where a half is free.  With every half taken by
-// coders the sorts starve (compress fell from 1.4 to 0.35 GB/s in a saturated pipeline, profiles/r2e_call_e.log), so a caller that keeps
+// coders the sorts starve in a saturated pipeline, so a caller that keeps
 // both directions in flight can leave a share of the SMs to the sorts.  Host-side counting semaphore; a launch waits for its CTAs' worth.
 struct CoderSlots {
     static int limit() { static const int v = [] { const char *e = getenv("BSCB200_CODER_SLOTS"); int k = e ? atoi(e) : 0; return k >= 8 ? k : 0; }(); return v; }
@@ -266,10 +276,9 @@ __device__ __forceinline__ void signal_done(const DoneSignal &s)
 __device__ __forceinline__ u32 lanemask_lt() { u32 m; asm("mov.u32 %0, %%lanemask_lt;" : "=r"(m)); return m; }
 
 // Lanes of the warp that hold the same `bits`-bit digit as this lane, from one ballot per digit bit (all 32 lanes must call it).
-// A/B on the B200 against __match_any_sync (profiles/r2d_call_d.log): as a DEPENDENT operation match.any costs 85 / 217 / 393 cycles for
-// 4 / 16 / 32 distinct values, but its THROUGHPUT with many warps in flight is better than 8 ballots + 8 selects -- rs_onesweep 2712 ->
-// 2490 GB/s, unbwt_lf 1032 -> 870 GB/s with ballots -- so the multisplits keep match.any; the grid-stride histogram (one item per
-// thread and iteration, little else to overlap with) gained 18 % from the ballots and keeps them.
+// Against __match_any_sync: as a DEPENDENT operation match.any is slow for many distinct values, but its THROUGHPUT with many warps in
+// flight is better than 8 ballots + 8 selects, so the multisplits (rs_onesweep, unbwt_lf) keep match.any; the grid-stride histogram
+// (one item per thread and iteration, little else to overlap with) is faster with the ballots and keeps them.
 __device__ __forceinline__ u32 warp_peers(u32 d, int bits)
 {
     u32 m = 0xffffffffu;

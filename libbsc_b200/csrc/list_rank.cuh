@@ -38,7 +38,7 @@ __global__ void __launch_bounds__(256) lr_jump(u64 *pair, u32 n, u32 *flags, int
             more = !(d & LR_DONE);
         }
     }
-    // ONE store per CTA: two million threads storing to the same word took 0.12 ms per round (profiles/r2g_call_g.log)
+    // ONE store per CTA: two million threads storing to the same word serialise
     if (__syncthreads_or(more) && threadIdx.x == 0) flags[round] = 1;
 }
 

@@ -243,7 +243,7 @@ static const QTables *get_tables(Ctx *ctx)
     return d;
 }
 
-// Coder ids (libbsc.h:60-62): 1 static, 2 adaptive, 3 fast -- all three run on the device (parity on the B200: profiles/r2a_call_a.log).
+// Coder ids (libbsc.h:60-62): 1 static, 2 adaptive, 3 fast -- all three run on the device.
 static int coder_gate(int coder) { return (coder >= 1 && coder <= 3) ? LIBBSC_NO_ERROR : LIBBSC_BAD_PARAMETER; }
 static_assert(QF_COLD <= 2 * (size_t)COLD_PAD, "the fast coder's cold counters must fit the per-stream model allocation");
 
@@ -278,7 +278,7 @@ static int decoder_layout_by_load(int device)
     static std::atomic<int> mode[16];
     const int load = CodersInFlight::now(device);
     std::atomic<int> &m = mode[device & 15];
-    if (load * Q_MAX_SUB > B200_SMS) m.store(5);
+    if (load * Q_MAX_SUB > (int)device_sms(device)) m.store(5);
     else if (load <= 4) m.store(4);
     const int v = m.load();
     return v ? v : 4;
@@ -377,8 +377,8 @@ int stage_coder_compress(Ctx *ctx, const u8 *d_in, u8 *d_out, int n_, int coder,
         LAUNCH(ctx, q_rank_tile, ceil_div(total_tiles, 4), 128, 0, run_sym, run_rank, d_sb, (u32)nBlocks, total_tiles, next_tab);
     }
     // The counter file of the static coder is the "diet" layout (qlfc_decoder6.cuh: 106 KB + 5.6 KB of pipe state for the encoder,
-    // 110 KB for the decoder), so that TWO coder CTAs share an SM: a coder CTA keeps one scheduler a third busy (ncu: 0.27-0.35
-    // issue slots per cycle, profiles/r2a_ncu_coder_kernels_4MiB.txt), and a second stream on the SM costs the first one ~15 %.
+    // 110 KB for the decoder), so that TWO coder CTAs share an SM: a coder CTA keeps one scheduler only partly busy (it waits on a
+    // dependency chain), so a second stream on the SM costs the first one little.
     static_assert(((sizeof(CoderSmemT<LayoutEncDiet>) + 15) & ~(size_t)15) + sizeof(EncPipe) <= 232448 / 2 - 1024, "two encoders must fit one SM");
     static_assert(3 * (((sizeof(CoderSmemT<LayoutEncDietTG>) + 15) & ~(size_t)15) + sizeof(EncPipe) + 1024) <= 232448, "three encoders without resident state tables must fit one SM");
     static_assert(4 * (((sizeof(CoderSmemT<LayoutEncDiet4>) + 15) & ~(size_t)15) + sizeof(EncPipe) + 1024) <= 232448, "four encoders per SM");
@@ -560,12 +560,12 @@ int stage_coder_decompress(Ctx *ctx, const u8 *d_in, int in_size, u8 *d_out, int
                 const int n_hi = coder_split_point(packed, list, nlist);
                 // Streams per SM = how much of the counter file is resident (qlfc_decoder6.cuh).  BSCB200_DEC_PER_SM = 2: LayoutDiet (state
                 // tables resident, 110 KB); 3: LayoutDietTG (tables through L1, 71 KB); 4: LayoutDiet4 (55 KB, rank exponent 4 row-wise);
-                // 5: LayoutDiet5 (39 KB; 11 % slower per stream when alone, 836 against 807 MB/s in a full pipeline, profiles/r2j_call_j.log).
+                // 5: LayoutDiet5 (39 KB; slower per stream when alone, more streams in flight in a full pipeline).
                 // Default: by load, with hysteresis -- 4 per SM while every stream of the blocks in coder stages on this device can have an SM
-                // share of its own choosing (<= 18 blocks = 144 streams: a caller with a handful of blocks wants the short latency); 5 per SM
+                // share of its own choosing (blocks x 8 streams <= the device's SMs, 16 blocks on an H100: a caller with a handful of blocks
+                // wants the short latency); 5 per SM
                 // once streams have to share SMs anyway, and then until the device has drained to 4 blocks: a MIX of 55 KB and 39 KB CTAs packs
-                // an SM badly (a load hovering around the old threshold of 37 blocks gave 786 MB/s against 807 / 836 for all-4 / all-5,
-                // profiles/r2j_call_j.log).
+                // an SM badly (a load hovering around a single threshold was slower than either layout alone in a full pipeline).
                 static const int forced = [] { const char *e = getenv("BSCB200_DEC_PER_SM"); const int v = e ? atoi(e) : 0; return (v >= 2 && v <= 5) ? v : 0; }();
                 const int per_sm = forced ? forced : decoder_layout_by_load(ctx->device);
                 auto launch = [&](auto kernel, size_t smem) {

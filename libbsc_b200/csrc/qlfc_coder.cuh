@@ -4,10 +4,8 @@
 // Why this looks the way it does.  One coder stream is a strictly serial recurrence (every binary
 // decision reads three adaptive counters whose addresses depend on the previous decisions, then
 // updates them and the range coder).  The format allows only <= 8 streams per block
-// (coder.cpp:52-59), so per-stream LATENCY is everything.  Measured history (profiles/):
-//   r1a  counters in global memory                 ~370 cycles / decision (each load an L2 round trip)
-//   r1b  16 K-entry shared-memory caches           ~200 cycles / decision (working set did not fit)
-// so the counter file is now laid out for shared memory: one SM per stream holds
+// (coder.cpp:52-59), so per-stream LATENCY is everything.  Counters in global memory cost an L2 round
+// trip per load, and small shared-memory caches in front of them did not hold the working set, so the counter file is now laid out for shared memory: one SM per stream holds
 //
 //   * state tables                                  40 KB  (tables.h data, qlfc_tables.inc)
 //   * first-bit, unary-exponent (index < 8) and model-wide shared counters      25 KB

@@ -2,10 +2,9 @@
 // of the counter file as a template parameter so that it fits TWO streams per SM.  Included by qlfc.cu after qlfc_lanes.cuh; also
 // compiled for the host (tools/qdec3_host.cpp), where the 32 lanes are emulated and the output is compared with reference streams.
 //
-// Why two per SM: the decoder is a serial recurrence (the context of every decision depends on the previous decisions); ncu on the
-// B200 (profiles/r2a_ncu_coder_kernels_4MiB.txt) shows one warp issuing 0.35 instructions per cycle on ONE of the SM's four
-// schedulers -- 2.88 cycles per instruction, of which 1.32 are fixed-latency dependency waits -- so a second stream on the same SM
-// is almost free (measured: 15 % slower per stream, profiles/r2b_call_b.log).  The "diet" layout keeps resident only what is hot:
+// Why two per SM: the decoder is a serial recurrence (the context of every decision depends on the previous decisions); one warp
+// issues well under one instruction per cycle on ONE of the SM's four schedulers -- most of its cycles are fixed-latency
+// dependency waits -- so a second stream on the same SM costs the first one little.  The "diet" layout keeps resident only what is hot:
 //     state tables 40 KB | first-bit / exponent / shared counters 25 KB | rank mantissa trees for exponents 1..4 (30 nodes
 //     per state / symbol) 30 KB | run mantissa trees for exponents 1..3 | staged rows
 // = 110 KB.  Everything else (rank exponent 5, the escape bank, long runs) is used ROW-wise from HBM: the counters one run can
@@ -244,8 +243,7 @@ template <class LY> QD3_FN u32 qd6_step(const SM3 &sm, Rc3 &rc, u32 p)
 
 
 // Counter moves (p * M + K) >> 12 as in qlfc_coder.cuh.  IMAD takes ONE immediate (the addend), so ptxas re-materialises
-// every multiplier with a MOV in front of every use -- 6 of the 53 instructions of a mantissa decision in q_decode3<1>
-// (profiles/r1h), and it folds any constant it can see.  The multipliers of the four hot decision classes are therefore
+// every multiplier with a MOV in front of every use -- a visible share of the instructions of a mantissa decision -- and it folds any constant it can see.  The multipliers of the four hot decision classes are therefore
 // LOADED (from a small table in global memory) into registers once per stream: 24 registers, no MOVs.
 QD3_FN constexpr int qd6_hot(int k) { return k == K_RANK_T ? 0 : k == K_RANK_E ? 1 : k == K_RANK_M ? 2 : k == K_RUN_T ? 3 : -1; }
 constexpr int QD6_HOT_CLASSES[4] = {K_RANK_T, K_RANK_E, K_RANK_M, K_RUN_T};

@@ -28,9 +28,9 @@
 // to each other; the coder consumes up to the minimum of the four progress counters.  A batch is cut
 // short so that its records never exceed half the ring.
 //
-// History of the critical model warp's instruction count per run (ncu, profiles/): one warp doing
-// everything 530 -> 2 model warps 205 -> vector prologue 170 -> 4 model warps, lane per decision of one
-// run ~100 -> lane per decision of 32 runs (this file) ~25; the range-coder warp is now the limit.
+// The critical model warp's instruction count per run fell with each step -- one warp doing everything, two model warps, a
+// vector prologue, four model warps with a lane per decision of one run, a lane per decision of 32 runs (this file) -- until
+// the range-coder warp became the limit.
 #pragma once
 
 #define QE_RING 1024
@@ -146,8 +146,8 @@ __device__ __forceinline__ int enc_resolve(CoderSmemT<LY> &S, bool act, u32 x, b
 __device__ __forceinline__ u32 enc_window(u32 prev_rev, u32 cur_rev, u32 lane) { return (u32)((((u64)prev_rev << 32) | cur_rev) >> (32u - lane)); }
 
 // LY: layout of the counter file (qlfc_decoder6.cuh).  The product instantiates LayoutEncDiet: fewer mantissa rows resident, 106 KB
-// + 5.6 KB of pipe state, so that two six-warp encoders share an SM (same time per stream as the 205 KB layout when alone: 682 ms
-// per 64 MiB block, profiles/r2a_call_a.log).  (A one-multiply-add form of the range recurrence was tried in round 2: 707 vs 682 ms.)
+// + 5.6 KB of pipe state, so that two six-warp encoders share an SM (same time per stream as the 205 KB layout when alone).
+// (A one-multiply-add form of the range recurrence was tried and was slower.)
 // MINB: encoder CTAs per SM the REGISTER budget must allow (192 threads: 122 registers fit two CTAs, <= 112 three, <= 80 four)
 template <class LY, int MINB> __global__ void __launch_bounds__(QE_THREADS, MINB) q_encode5(const u32 *__restrict__ run_pos, const u8 *__restrict__ run_sym, const u8 *__restrict__ run_rank,
                                                     SubBlock *__restrict__ sbs, const u8 *__restrict__ mtf_all, short *__restrict__ cold_all,

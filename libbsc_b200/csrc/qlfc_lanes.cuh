@@ -2,8 +2,8 @@
 // coder qlfc_adaptive.cuh, fast coder qlfc_fast.cuh): the shared-memory image accessor SM3, the range-decoder registers Rc3, the
 // per-lane registers Qd3Lane, and the QD3_* macros that let THE SAME SOURCE compile for the host (tools/qdec3_host.cpp, QD3_HOST):
 // there the 32 lanes are emulated one after the other, so the lane logic is checked bit-for-bit against the reference's streams on
-// the CPU (tests/test_qdec3_host.py).  (Round 1 kept three more decoder generations in this file; they lost the A/B on the B200
-// -- profiles/r1h_decoder_ab.txt, profiles/r2a_call_a.log -- and are gone.)
+// the CPU (tests/test_qdec3_host.py).  (Three more decoder generations
+// once lived in this file; they lost the A/B and are gone.)
 #pragma once
 
 #include <cstddef>

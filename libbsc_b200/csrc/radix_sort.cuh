@@ -128,7 +128,7 @@ __device__ __forceinline__ u32 rs_block_excl_scan(u32 v, u32 *tmp, u32 lane, u32
 }
 
 // MINB = CTAs per SM the register budget is cut for: 3 -> 80 registers (37 % occupancy), 4 -> 64 registers without spills (50 %); four
-// 56 KB CTAs fill the 228 KB of an SM.  A/B on the B200: profiles/r2j_*.
+// 56 KB CTAs fill the 228 KB of an SM.
 template <typename K, bool HAS_VAL, class Src, int MINB>
 __global__ void __launch_bounds__(RS_THREADS, MINB)
 rs_onesweep(Src src, K *__restrict__ kout, u32 *__restrict__ vout, u32 n, int shift, int bits,
@@ -367,10 +367,10 @@ rs_onesweep_tma(const K *__restrict__ kin, const u32 *__restrict__ vin, K *__res
 }
 
 // ---- host driver ---------------------------------------------------------------------------
-// BSCB200_SORT_TMA=1: passes over materialised keys through rs_onesweep_tma.  A/B on the B200 (profiles/r2e_call_e.log, r2e_ncu_sort_stalls.txt):
-// the TMA-staged persistent kernel runs at 1757 GB/s against 2490 GB/s for rs_onesweep -- a persistent CTA holds the id of its PREFETCHED
+// BSCB200_SORT_TMA=1: passes over materialised keys through rs_onesweep_tma.  The TMA-staged
+// persistent kernel is slower than rs_onesweep -- a persistent CTA holds the id of its PREFETCHED
 // tile while it still works on the current one, so that tile's aggregate reaches the look-back a whole tile time later and the chain of
-// waits grows (long_scoreboard + branch_resolving 12.4 of 24.5 cycles per instruction); it also takes 109 KB of shared memory per CTA, which
+// waits grows (long-scoreboard and branch-resolving stalls dominate); it also takes 109 KB of shared memory per CTA, which
 // no SM half next to a coder CTA can give.  So it is not the default; it stays selectable and parity-tested.
 static inline int rs_min_blocks() { static const int v = [] { const char *e = getenv("BSCB200_SORT_OCC"); return (e && e[0] == '3') ? 3 : 4; }(); return v; }
 static inline bool rs_use_tma() { static const bool on = [] { const char *e = getenv("BSCB200_SORT_TMA"); return e && e[0] == '1'; }(); return on; }
@@ -395,7 +395,7 @@ static int rs_sort(Ctx *ctx, FirstSrc first, K *const k[2], u32 *const v[2], u32
     u64 *lookback = (u64 *)((u8 *)scratch + align_up(sizeof(u32) * 256 * RS_MAX_PASSES + sizeof(u32) * 64, 256));
     CUDA_TRY(cudaMemsetAsync(scratch, 0, rs_scratch_bytes(n, passes.count), ctx->stream));
 
-    u32 hgrid = min(tiles, (u32)(B200_SMS * 8));
+    u32 hgrid = min(tiles, device_sms(ctx->device) * 8);
     const double pass_bytes = 2.0 * (double)n * (sizeof(K) + (HAS_VAL ? 4 : 0));   // read + write of every element
     PROF_BYTES(ctx, (double)n * sizeof(K));
     LAUNCH(ctx, (rs_hist1<FirstSrc>), hgrid, RS_THREADS, 0, first, n, (int)passes.shift[0], (int)passes.bits[0], ghist);
@@ -424,7 +424,7 @@ static int rs_sort(Ctx *ctx, FirstSrc first, K *const k[2], u32 *const v[2], u32
             LAUNCH_NAMED(ctx, "rs_onesweep", k_next, tiles, RS_THREADS, smem,
                    src, k[dst], v[dst], n, (int)passes.shift[p], (int)passes.bits[p], ghist + 256 * p, hnext, s2, b2, counters + p, lb);
         } else {
-            const u32 grid = min(tiles, (u32)(B200_SMS * 2));                // persistent: two CTAs per SM, each loops over tiles
+            const u32 grid = min(tiles, device_sms(ctx->device) * 2);                // persistent: two CTAs per SM, each loops over tiles
             LAUNCH(ctx, (rs_onesweep_tma<K, HAS_VAL>), grid, RS_THREADS, smem_tma,
                    (const K *)k[dst ^ 1], (const u32 *)v[dst ^ 1], k[dst], v[dst], n, tiles, (int)passes.shift[p], (int)passes.bits[p], ghist + 256 * p, hnext, s2, b2, counters + p, lb);
         }

@@ -242,7 +242,7 @@ int stage_st_decode(Ctx *ctx, u8 *d_T, int n_, int k, int index_)
     CUDA_TRY(cudaMemsetAsync(small, 0, sizeof(u32) * 128, ctx->stream));
     CUDA_TRY(cudaMemsetAsync(rec, 0, sizeof(u64) * (size_t)n, ctx->stream));
 
-    LAUNCH(ctx, unbwt_hist, min(ceil_div(n, 256 * 64), (u32)(B200_SMS * 8)), 256, 0, Lp, n, hist);
+    LAUNCH(ctx, unbwt_hist, min(ceil_div(n, 256 * 64), device_sms(ctx->device) * 8), 256, 0, Lp, n, hist);
     LAUNCH(ctx, unbwt_scan256, 1, 32, 0, hist);
     PROF_BYTES(ctx, 5.0 * n);
     LAUNCH(ctx, unbwt_lf<false>, lf_tiles, LF_THREADS, 0, Lp, n, n, hist, hist + 256, lb, LF);

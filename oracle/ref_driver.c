@@ -7,9 +7,7 @@
  * When the host has more threads than there are blocks, the CLI leaves FEATURE_MULTITHREADING on, but
  * its intra-block OpenMP regions only get threads if nested parallelism is enabled, which the CLI does
  * not do.  refdrv_set_nested(1) enables two active levels with inner teams of max_threads / nBlocks
- * threads.  Measured on the B200 box's host (Xeon 8562Y+, 64 threads): 18 blocks, nested, 54 threads:
- * 134.7 MB/s round trip; 16 blocks, stock, 16 threads: 145.6 MB/s (profiles/r1h, r1g) -- nesting does not
- * help the reference, so the default is the stock CLI behaviour (the faster configuration).
+ * threads.  Nesting was measured not to help the reference, so the default is the stock CLI behaviour.
  * Used by bench.py for the `cpu_baseline` object and for `--impl reference`.
  * Links against libbsc_ref.so only (no product code, no oracle port).
  */

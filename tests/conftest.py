@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box via gpurun)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
 
 
 @pytest.fixture(scope="session")
@@ -46,5 +46,5 @@ def bsc():
     import libbsc_b200
     L = libbsc_b200.lib()                                  # a missing / unloadable library is an ERROR, never a skip
     if L.bsc_init(3) == -8:                                # LIBBSC_GPU_NOT_SUPPORTED: no CUDA device on this machine
-        pytest.skip("no CUDA device (gpu-marked tests run on the B200 box)")
+        pytest.skip("no CUDA device (gpu-marked tests need an H100)")
     return libbsc_b200.Bsc(features=3)

@@ -1,16 +1,20 @@
 """The `bsc1` file container and the block scheduler of libbsc_b200/cli/bsc_b200.cpp (SURVEY.md 8f #3).
 
 CPU part: the same CLI source is built against the UNMODIFIED reference library (-DBSCB200_CLI_REF: identical block API, no
-GPU) and its archives are compared with the reference's own CLI (oracle/_ref/bsc, built by oracle/Makefile from
-/root/reference/bsc.cpp): byte-identical containers when both write blocks in order (`bsc -t`), and each side decodes the
+GPU) and its archives are compared with the reference's own CLI (oracle/_ref/bsc, built by oracle/Makefile from the
+reference's bsc.cpp): byte-identical containers when both write blocks in order (`bsc -t`), and each side decodes the
 other's archives.  That pins the container logic, option handling and the in-order writer without a GPU.
-GPU part: the product binary libbsc_b200/bsc_b200 round-trips a file and
-produces the bytes of the reference CLI."""
+GPU part: the product binary libbsc_b200/bsc_b200 round-trips a file and produces the bytes of the reference CLI (its
+archive's size and SHA-256, tests/golden/reference_results.json)."""
+import hashlib
+import json
 import os
 import subprocess
 
 import numpy as np
 import pytest
+
+import reference_inputs as ri
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SRC = os.path.join(ROOT, "libbsc_b200", "cli", "bsc_b200.cpp")
@@ -128,14 +132,13 @@ def test_reader_undoes_reference_filters(clis, gen):
 @pytest.mark.gpu
 def test_product_cli_round_trip_on_gpu(gen, tmp_path):
     path, arch, back = str(tmp_path / "in.bin"), str(tmp_path / "a.bsc"), str(tmp_path / "back.bin")
-    gen.text(2, 40 << 20).tofile(path)
-    _run(PRODUCT, "e", path, arch, "-b8", "-j5")
+    ri.cli_input(gen).tofile(path)
+    _run(PRODUCT, "e", path, arch, *ri.CLI_OPTS, "-j5")
     _run(PRODUCT, "d", arch, back, "-j5")
     assert open(back, "rb").read() == open(path, "rb").read()
-    if os.path.exists(REFCLI):
-        theirs = str(tmp_path / "t.bsc")
-        _run(REFCLI, "e", path, theirs, "-b8", "-p", "-t")
-        assert open(arch, "rb").read() == open(theirs, "rb").read()
+    ours = open(arch, "rb").read()
+    gold = json.load(open(os.path.join(ROOT, "tests", "golden", "reference_results.json")))["cli_archive"]   # `bsc e in out -b8 -p -t`
+    assert {"size": len(ours), "sha256": hashlib.sha256(ours).hexdigest()} == gold
 
 
 @pytest.mark.gpu

@@ -1,6 +1,6 @@
 """GPU parity tests of the ADAPTIVE (coder id 2, csrc/qlfc_adaptive.cuh) and FAST (coder id 3, csrc/qlfc_fast.cuh) QLFC coders
 through the C ABI (SURVEY 8(f) #1): byte-identical streams, containers and blocks against the reference, and decoding of the
-reference's streams.  Both coders first passed here on the B200 in round 2 (profiles/r2a_call_a.log); they are ungated since."""
+reference's streams."""
 import numpy as np
 import pytest
 

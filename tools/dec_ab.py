@@ -2,7 +2,7 @@
 """tools/dec_ab.py -- timing of the QLFC coder kernels on ONE block (CUDA events around every launch), round trip checked.
     python tools/dec_ab.py [MiB]
 (Round 2's A/B of the decoder generations and encoder variants used this script with BSCB200_QDEC / BSCB200_QENC at commit 4a20aea:
-profiles/r2a_call_a.log; the losers are gone and so are the switches.)"""
+the losers are gone and so are the switches.)"""
 import os
 import subprocess
 import sys

@@ -1,7 +1,7 @@
 #!/usr/bin/env python3
-"""tools/ncu_summary.py -- condense an .ncu-rep (read here with `ncu -i`) into the lines profiles/ keeps: duration, issue statistics,
+"""tools/ncu_summary.py -- condense an .ncu-rep (read here with `ncu -i`) into a few lines: duration, issue statistics,
 warp stall reasons per issued instruction, instruction / branch counts, launch shape, DRAM bytes when the capture has them.
-    python tools/ncu_summary.py gpurun_out/x.ncu-rep [...] > profiles/rN_x.txt"""
+    python tools/ncu_summary.py x.ncu-rep [...] > x.txt"""
 import csv
 import subprocess
 import sys

@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
 """tools/one_block.py -- compress + decompress ONE synthetic block through the device-resident ABI.
-Small driver for `ncu` captures (profiles/): python tools/one_block.py [MiB] [sorter]"""
+Small driver for one-block captures: python tools/one_block.py [MiB] [sorter]"""
 import os
 import sys
 

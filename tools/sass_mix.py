@@ -1,7 +1,7 @@
 #!/usr/bin/env python3
 """tools/sass_mix.py -- per-kernel instruction mix of the built library's SASS (runs without a GPU): total instructions, TMA bulk copies
 (UBLKCP) and mbarrier operations (SYNCS), 128- / 64-bit global loads and stores, match.any, shuffles.
-    python tools/sass_mix.py > profiles/r2_sass_instruction_mix.txt"""
+    python tools/sass_mix.py > sass_instruction_mix.txt"""
 import collections
 import os
 import re
@@ -26,7 +26,7 @@ for line in sass.splitlines():
 names = list(per)
 dem = subprocess.run(["cu++filt"] + names, capture_output=True, text=True).stdout.split("\n")
 cols = ["total", "UBLKCP", "SYNCS", "LDG.128", "LDG.64", "STG.128", "STG.64", "MATCH", "SHFL", "ATOMS"]
-print("SASS of libbsc_b200/libbsc_b200.so (sm_100a): instruction counts per kernel (cuobjdump -sass, tools/sass_mix.py); %d kernels" % len(names))
+print("SASS of libbsc_b200/libbsc_b200.so (sm_90a): instruction counts per kernel (cuobjdump -sass, tools/sass_mix.py); %d kernels" % len(names))
 print("%-100s " % "kernel" + " ".join("%7s" % c for c in cols))
 for n, d in sorted(zip(names, dem), key=lambda x: -per[x[0]]["total"]):
     short = re.sub(r"\((const |unsigned |<unnamed>::|void|int|short|DoneSignal|[\w\*&, ])*\)$", "", d).replace("<unnamed>::", "").replace("void ", "")[:98]

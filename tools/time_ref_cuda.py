@@ -3,9 +3,9 @@
 same host-pointer entry points (bsc_bwt_encode / bsc_bwt_decode / bsc_st_encode: H2D + kernels + D2H inside both timings).
 
 The reference side is oracle/_ref/libbsc_refcuda.so: the unmodified reference compiled by oracle/Makefile with -DLIBBSC_CUDA_SUPPORT for
-sm_100 (SURVEY 8c "second baseline"; rows a3 / a6 / a8).  Both sides get `reps` warm calls; best and median wall times are reported,
+sm_90 (SURVEY 8c "second baseline"; rows a3 / a6 / a8).  Both sides get `reps` warm calls; best and median wall times are reported,
 plus our own kernel-only time (CUDA events around every launch of the stage).  Outputs are compared byte for byte.
-    python tools/time_ref_cuda.py [reps] > gpurun_out/ref_cuda.json"""
+    python tools/time_ref_cuda.py [reps] > ref_cuda.json"""
 import ctypes
 import json
 import os
@@ -152,4 +152,4 @@ rows.append({"stage": "bsc_st_decode k=6 32 MiB G_skew (reference: CPU, OpenMP)"
 for r in rows:
     r["speedup_best"] = round(r["ref_cuda_ms_best"] / r["ours_ms_best"], 2)
     sys.stderr.write("%-58s ref %9.1f ms   ours %9.1f ms (kernels %8.1f)   x%.2f\n" % (r["stage"], r["ref_cuda_ms_best"], r["ours_ms_best"], r["ours_kernels_only_ms"], r["speedup_best"]))
-print(json.dumps({"what": "reference CUDA build (libcubwt 1.6.1 / st.cu, sm_100 SASS) vs libbsc_b200, host-pointer calls, wall clock incl. H2D/D2H", "reps": reps, "rows": rows}, indent=1))
+print(json.dumps({"what": "reference CUDA build (libcubwt 1.6.1 / st.cu, sm_90 SASS) vs libbsc_b200, host-pointer calls, wall clock incl. H2D/D2H", "reps": reps, "rows": rows}, indent=1))

@@ -1,6 +1,6 @@
 // tools/warp_latency.cu -- dependent-chain latency (cycles) of the warp primitives the QLFC coder leans on,
 // measured with ONE resident warp (the situation of a coder warp: nothing else hides latency).
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o gpurun_out/warp_latency tools/warp_latency.cu && gpurun_out/warp_latency
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o warp_latency tools/warp_latency.cu && ./warp_latency
 #include <cstdio>
 #include <cuda_runtime.h>
 
