@@ -53,7 +53,9 @@ int bsc_init_full(int features, void *(*malloc_fn)(size_t), void *(*zero_malloc_
 
 /* libbsc/libbsc.h:118 ; libbsc.cpp:213-338.  output holds n + 28 bytes; input may equal output.
  * bsc_compress: LZP (lzpHashSize/lzpMinLen != 0) is outside the replaced path: LIBBSC_NOT_SUPPORTED.
- * bsc_decompress: blocks with an LZP stage are accepted (the inverse stage runs on the host after the GPU stages). */
+ * bsc_decompress: blocks with an LZP stage are accepted (the inverse stage runs on the host after the GPU stages).
+ * Block size: n <= 1 GiB (1073741824).  The reference also accepts in-place calls up to 2146435072 bytes; here those return
+ * LIBBSC_NOT_SUPPORTED (out of place, n > 1 GiB is LIBBSC_BAD_PARAMETER as in the reference). */
 int bsc_compress(const unsigned char *input, unsigned char *output, int n, int lzpHashSize, int lzpMinLen, int blockSorter, int coder, int features);
 /* libbsc/libbsc.h:128 ; libbsc.cpp:68-81 */
 int bsc_store(const unsigned char *input, unsigned char *output, int n, int features);
@@ -107,6 +109,13 @@ int bscb200_coder_decompress(const unsigned char *input, int inputSize, unsigned
 void              *bscb200_ctx_create(int device, void *cuda_stream);
 void               bscb200_ctx_destroy(void *ctx);
 int                bscb200_ctx_reserve(void *ctx, long long bytes);
+/* Bounds the forward BWT's working set on this context: whenever the standard sorter would need more than `bytes` (about 58 n + 64 MB
+ * for a block of n), the sort runs in batches of B = (bytes - 16 n) / 32 entries in about 16 n + 32 B bytes.  Same results either way.
+ * B is at least max(65536, n / 64): every key range of the initial sort and of an oversized group rescans its segment, so the work
+ * grows with n / B, and the floor keeps it within about 64 passes over the block per such segment.  Smaller batches cost time: see
+ * DESIGN.md 4.2 for measured times.  0 (the default) = no bound; negative = LIBBSC_BAD_PARAMETER.  Block sorters 3..8 ignore it.
+ * The block-size limits do not change: blocks above 1 GiB are still LIBBSC_NOT_SUPPORTED. */
+int                bscb200_ctx_set_sort_budget(void *ctx, long long bytes);
 int                bscb200_lzp_decompress_host(const unsigned char *input, int n, unsigned char *output, int outputCapacity, int lzpHashSize, int lzpMinLen);   /* inverse of the reference LZP stage (libbsc/lzp/lzp.h), host only */
 int                bscb200_lzp_compress_host(const unsigned char *input, unsigned char *output, int n, int lzpHashSize, int lzpMinLen, int features);   /* the reference LZP stage forward (libbsc/lzp/lzp.h), host only */
 int                bscb200_device_count(void);                    /* CUDA devices visible to the process */
@@ -124,7 +133,9 @@ int                bscb200_ctx_profile_report(void *ctx, char *buf, int cap);
 const char        *bscb200_version(void);
 
 /* Device-resident variants: all d_* pointers are device pointers on the context's device.
- * Same return values as their host-pointer counterparts. */
+ * Same return values as their host-pointer counterparts.  bscb200_compress_device takes n <= 1 GiB (LIBBSC_BAD_PARAMETER above);
+ * bscb200_bwt_encode_device takes any n >= 0, but the standard sorter needs about 58 n bytes, so above a few hundred MiB on an
+ * 80 GB card a context needs a sort budget (bscb200_ctx_set_sort_budget). */
 int bscb200_compress_device(void *ctx, const unsigned char *d_input, unsigned char *d_output /* n+28 */, int n, int blockSorter, int coder, int features);
 int bscb200_decompress_device(void *ctx, const unsigned char *d_input, int inputSize, unsigned char *d_output, int outputSize, int features);
 int bscb200_bwt_encode_device(void *ctx, unsigned char *d_T, int n, unsigned char *num_indexes /* host */, int *indexes /* host */);

@@ -54,6 +54,7 @@ _SIGNATURES = {
     "bscb200_ctx_create": ([ci, vp], vp),
     "bscb200_ctx_destroy": ([vp], None),
     "bscb200_ctx_reserve": ([vp, ctypes.c_longlong], ci),
+    "bscb200_ctx_set_sort_budget": ([vp, ctypes.c_longlong], ci),
     "bscb200_lzp_decompress_host": ([vp, ci, vp, ci, ci, ci], ci),
     "bscb200_lzp_compress_host": ([vp, vp, ci, ci, ci, ci], ci),
     "bscb200_device_count": ([], ci),
@@ -222,6 +223,10 @@ class DeviceCtx:
 
     def reserve(self, nbytes):
         return self.lib.bscb200_ctx_reserve(self.handle, nbytes)
+
+    def set_sort_budget(self, nbytes):
+        """Bound the forward BWT's working set to about `nbytes` (batched sort above it; 0 = no bound).  Returns 0 or BAD_PARAMETER."""
+        return self.lib.bscb200_ctx_set_sort_budget(self.handle, nbytes)
 
     def launches(self):
         return int(self.lib.bscb200_ctx_kernel_launches(self.handle))

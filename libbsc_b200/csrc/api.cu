@@ -238,6 +238,19 @@ size_t readable_prefix(const void *p, size_t want)
 
 bool sorter_valid(int s) { return s == 1 || (s >= 3 && s <= 8); }
 
+// Forward BWT of a block on this context, its sort in a shared slab: the standard sorter, or the batched one when the context's sort
+// budget (bscb200_ctx_set_sort_budget) is smaller than the standard working set.
+int bwt_encode_leased(Ctx *ctx, u8 *d_T, int n, unsigned char *num_indexes, int *indexes)
+{
+    if (ctx->sort_budget <= 0 || n <= 1 || (long long)need_bwt_encode((size_t)n) <= ctx->sort_budget) {
+        ScratchLease lease(ctx, need_bwt_encode((size_t)n));
+        return stage_bwt_encode(ctx, d_T, n, num_indexes, indexes);
+    }
+    const u32 B = bwt_batch_entries((u32)n, ctx->sort_budget);
+    ScratchLease lease(ctx, bwt_batched_bytes((u32)n, B));
+    return stage_bwt_encode_batched(ctx, d_T, n, num_indexes, indexes, B);
+}
+
 // ---------------------------------------------------------------------------------------------
 // device-resident block compress / decompress
 // ---------------------------------------------------------------------------------------------
@@ -277,11 +290,8 @@ int compress_dev(Ctx *ctx, const u8 *d_in, int n, u8 *d_out, int blockSorter, in
     CUDA_TRY(cudaMemcpyAsync(work, d_in, (size_t)n, cudaMemcpyDeviceToDevice, ctx->stream));
 
     int indexes[256]; unsigned char num_indexes = 0; int index;
-    {
-        ScratchLease lease(ctx, blockSorter == 1 ? need_bwt_encode(n) : need_st_encode(n));      // the sort's ~58 n live in a shared slab
-        if (blockSorter == 1) index = stage_bwt_encode(ctx, work, n, &num_indexes, indexes);
-        else index = stage_st_encode(ctx, work, n, blockSorter);
-    }
+    if (blockSorter == 1) index = bwt_encode_leased(ctx, work, n, &num_indexes, indexes);      // the sort's ~58 n live in a shared slab
+    else { ScratchLease lease(ctx, need_st_encode(n)); index = stage_st_encode(ctx, work, n, blockSorter); }
     if (orig_n < 64 * 1024) num_indexes = 0;              // libbsc.cpp:303
     if (index < 0) { A.release(mark); return index; }
 
@@ -515,8 +525,7 @@ int bsc_bwt_encode(unsigned char *T, int n, unsigned char *num_indexes, int *ind
         ctx->arena.reserve((size_t)n + 4096);
         u8 *d = ctx->arena.get<u8>((size_t)n + 64);
         if (n > 0) CUDA_TRY(cudaMemcpyAsync(d, T, (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
-        ScratchLease lease(ctx, need_bwt_encode(n));
-        int r = stage_bwt_encode(ctx, d, n, num_indexes, indexes);
+        int r = bwt_encode_leased(ctx, d, n, num_indexes, indexes);
         if (r >= 0 && n > 0) { CUDA_TRY(cudaMemcpyAsync(T, d, (size_t)n, cudaMemcpyDeviceToHost, ctx->stream)); ctx->sync(); }
         return r;
     });
@@ -698,6 +707,14 @@ int bscb200_ctx_reserve(void *ctx, long long bytes)
     Ctx *c = (Ctx *)ctx;
     return guarded(c, [&]() { CUDA_TRY(cudaSetDevice(c->device)); c->arena.reset(); c->arena.reserve((size_t)bytes); return 0; });
 }
+// Bounds the forward BWT's working set on this context: it sorts in batches whenever the standard sorter would need more than `bytes`
+// (0 = no bound).  Block sorters 3..8 ignore it.
+int bscb200_ctx_set_sort_budget(void *ctx, long long bytes)
+{
+    if (!ctx || bytes < 0) return LIBBSC_BAD_PARAMETER;
+    ((Ctx *)ctx)->sort_budget = bytes;
+    return LIBBSC_NO_ERROR;
+}
 // Per-context workspace: the staged block + the coder stage (the inverse BWT reuses the coder's space).  The sort stages work in
 // the device-wide scratch slabs (scratch pool above), which is what lets dozens of blocks be in flight per GPU.
 long long bscb200_workspace_bytes(int n, int blockSorter)
@@ -773,7 +790,7 @@ int bscb200_decompress_device(void *ctx, const unsigned char *d_input, int input
 int bscb200_bwt_encode_device(void *ctx, unsigned char *d_T, int n, unsigned char *num_indexes, int *indexes)
 {
     Ctx *c = (Ctx *)ctx;
-    return guarded(c, [&]() { c->arena.reset(); ScratchLease lease(c, need_bwt_encode((size_t)n)); return stage_bwt_encode(c, d_T, n, num_indexes, indexes); });
+    return guarded(c, [&]() { c->arena.reset(); return bwt_encode_leased(c, d_T, n, num_indexes, indexes); });
 }
 int bscb200_bwt_decode_device(void *ctx, unsigned char *d_T, int n, int index)
 {

@@ -109,6 +109,7 @@ struct Ctx {
     Arena        arena;                 // per-block state: staged block, coder stage, inverse BWT
     Scratch     *scratch = nullptr;     // held only while a sort stage runs (ScratchLease in api.cu); sort stages fall back to `arena`
     Arena       &sort_arena() { return scratch ? scratch->arena : arena; }
+    long long    sort_budget = 0;       // > 0: the forward BWT sorts in batches when its standard working set is larger (bscb200_ctx_set_sort_budget)
     u32         *h_mail = nullptr;      // pinned host mailbox (64 words) for small D2H read-backs
     u32         *d_mail = nullptr;      // device mailbox (64 words)
     u8          *h_stage = nullptr;     // pinned staging for host<->device block copies

@@ -5,6 +5,15 @@
 
 // Forward BWT in place (bsc_bwt_encode, bwt.cpp:178).  num_indexes/indexes are HOST pointers (may be NULL).
 int stage_bwt_encode(Ctx *ctx, u8 *d_T, int n, unsigned char *num_indexes, int *indexes);
+// The same result with a bounded working set (bwt_encode_batched.cu): sorts in batches of at most B entries (raised to
+// bwt_batch_floor(n) if smaller) and takes bwt_batched_bytes(n, B) from ctx->sort_arena(); d_T needs no padding or alignment.
+int stage_bwt_encode_batched(Ctx *ctx, u8 *d_T, int n, unsigned char *num_indexes, int *indexes, u32 B);
+size_t bwt_batched_bytes(u32 n, u32 B);
+// smallest batch: max(65536, n / BWT_BATCH_FLOOR_DIV), which bounds the passes over the block
+#define BWT_BATCH_FLOOR_DIV 64
+u32 bwt_batch_floor(u32 n);
+// batch entries that a working set of `budget` bytes allows at block length n (at least bwt_batch_floor(n), at most that or n)
+u32 bwt_batch_entries(u32 n, long long budget);
 // Inverse BWT in place (bsc_bwt_decode, bwt.cpp:283).
 int stage_bwt_decode(Ctx *ctx, u8 *d_T, int n, int index);
 // Sort transform of order k in place (bsc_st_encode, st.cpp:990; k = 3..8).
