@@ -42,8 +42,8 @@ extern "C" {
 #endif
 #define LIBBSC_BLOCKSORTER_BWT         1   /* 3..8 = ST3..ST8 */
 #define LIBBSC_CODER_QLFC_STATIC       1
-#define LIBBSC_CODER_QLFC_ADAPTIVE     2   /* experimental: LIBBSC_NOT_SUPPORTED unless BSCB200_ENABLE_ADAPTIVE=1 (csrc/qlfc_adaptive.cuh) */
-#define LIBBSC_CODER_QLFC_FAST         3   /* experimental: LIBBSC_NOT_SUPPORTED unless BSCB200_ENABLE_FAST=1 (csrc/qlfc_fast.cuh) */
+#define LIBBSC_CODER_QLFC_ADAPTIVE     2   /* csrc/qlfc_adaptive.cuh */
+#define LIBBSC_CODER_QLFC_FAST         3   /* csrc/qlfc_fast.cuh */
 
 /* ---- group 1: libbsc-compatible entry points -------------------------------------------- */
 
@@ -54,8 +54,12 @@ int bsc_init_full(int features, void *(*malloc_fn)(size_t), void *(*zero_malloc_
 /* libbsc/libbsc.h:118 ; libbsc.cpp:213-338.  output holds n + 28 bytes; input may equal output.
  * bsc_compress: LZP (lzpHashSize/lzpMinLen != 0) is outside the replaced path: LIBBSC_NOT_SUPPORTED.
  * bsc_decompress: blocks with an LZP stage are accepted (the inverse stage runs on the host after the GPU stages).
- * Block size: n <= 1 GiB (1073741824).  The reference also accepts in-place calls up to 2146435072 bytes; here those return
- * LIBBSC_NOT_SUPPORTED (out of place, n > 1 GiB is LIBBSC_BAD_PARAMETER as in the reference). */
+ * Block size: n <= 1 GiB (1073741824), and in place (input == output) up to 2146435072 bytes as in the reference; out of place,
+ * n > 1 GiB is LIBBSC_BAD_PARAMETER as in the reference.  An in-place block above 1 GiB is sorted in place with the batched forward
+ * BWT on a context of its own, in at most bscb200_inplace_bytes() = 18 n + 256 MiB of HBM, all of it freed when the call returns;
+ * LIBBSC_GPU_NOT_ENOUGH_MEMORY (nothing written) when the device has less free.  The caller's buffer is written only on success.
+ * Above 1 GiB the sort transforms (blockSorter 3..8) return LIBBSC_NOT_SUPPORTED: they need about 30 n to encode and 41 n to decode
+ * and have no bounded variant. */
 int bsc_compress(const unsigned char *input, unsigned char *output, int n, int lzpHashSize, int lzpMinLen, int blockSorter, int coder, int features);
 /* libbsc/libbsc.h:128 ; libbsc.cpp:68-81 */
 int bsc_store(const unsigned char *input, unsigned char *output, int n, int features);
@@ -114,7 +118,7 @@ int                bscb200_ctx_reserve(void *ctx, long long bytes);
  * B is at least max(65536, n / 64): every key range of the initial sort and of an oversized group rescans its segment, so the work
  * grows with n / B, and the floor keeps it within about 64 passes over the block per such segment.  Smaller batches cost time: see
  * DESIGN.md 4.2 for measured times.  0 (the default) = no bound; negative = LIBBSC_BAD_PARAMETER.  Block sorters 3..8 ignore it.
- * The block-size limits do not change: blocks above 1 GiB are still LIBBSC_NOT_SUPPORTED. */
+ * bscb200_compress_device keeps its 1 GiB limit; blocks above it go through the in-place bsc_compress. */
 int                bscb200_ctx_set_sort_budget(void *ctx, long long bytes);
 int                bscb200_lzp_decompress_host(const unsigned char *input, int n, unsigned char *output, int outputCapacity, int lzpHashSize, int lzpMinLen);   /* inverse of the reference LZP stage (libbsc/lzp/lzp.h), host only */
 int                bscb200_lzp_compress_host(const unsigned char *input, unsigned char *output, int n, int lzpHashSize, int lzpMinLen, int features);   /* the reference LZP stage forward (libbsc/lzp/lzp.h), host only */
@@ -125,6 +129,10 @@ int                bscb200_set_device(int device);                /* bind the ca
 long long          bscb200_workspace_bytes(int n, int blockSorter);   /* per-context workspace (~13 n + 64 MB): staged block + coder stage */
 long long          bscb200_workspace_bytes_decode(int n);         /* the same (kept for callers of the round-1 ABI) */
 long long          bscb200_scratch_bytes(int n, int blockSorter);  /* one device-wide sort slab (~58 n for BWT); BSCB200_SORT_SLABS of them per GPU (default 3) */
+/* HBM that an in-place bsc_compress of a block of n > 1 GiB, or bsc_decompress of one, takes at most: 18 n + 256 MiB (about 39 GB at
+ * n = 2146435072), none of it kept after the call.  Same for the three coders and with LZP.  Blocks of at most 1 GiB take the pooled path
+ * instead (bscb200_workspace_bytes + bscb200_scratch_bytes).  blockSorter 3..8: LIBBSC_NOT_SUPPORTED; bad arguments: LIBBSC_BAD_PARAMETER. */
+long long          bscb200_inplace_bytes(int n, int blockSorter, int coder);
 unsigned long long bscb200_ctx_kernel_launches(void *ctx);
 unsigned long long bscb200_total_kernel_launches(void);
 /* per-kernel CUDA-event timing of everything launched through ctx (bench.py's roofline leg) */

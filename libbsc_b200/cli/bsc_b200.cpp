@@ -39,6 +39,7 @@
 extern "C" {
 int bsc_init(int features);
 int bsc_compress(const unsigned char *input, unsigned char *output, int n, int lzpHashSize, int lzpMinLen, int blockSorter, int coder, int features);
+int bsc_store(const unsigned char *input, unsigned char *output, int n, int features);
 int bsc_block_info(const unsigned char *blockHeader, int headerSize, int *pBlockSize, int *pDataSize, int features);
 int bsc_decompress(const unsigned char *input, int inputSize, unsigned char *output, int outputSize, int features);
 }
@@ -46,10 +47,12 @@ static int bscb200_device_count(void) { return 1; }
 static long long bscb200_device_free_bytes(void) { return -1; }
 static long long bscb200_workspace_bytes(int, int) { return 0; }
 static long long bscb200_scratch_bytes(int, int) { return 0; }
+static long long bscb200_inplace_bytes(int, int, int) { return 0; }
 static void bscb200_release_pools(void) {}
 static int bscb200_set_device(int) { return 0; }
 #define LIBBSC_HEADER_SIZE 28
 #define LIBBSC_NO_ERROR 0
+#define LIBBSC_NOT_COMPRESSIBLE -3
 #define LIBBSC_NOT_SUPPORTED -4
 #else
 #include "../../include/libbsc_b200.h"
@@ -59,6 +62,7 @@ namespace {
 
 const unsigned char kSign[4] = {'b', 's', 'c', 0x31};
 enum { kFeatures = 1 | 2, kContextsFollowing = 1, kContextsPreceding = 2, kRecordBytes = 10 };
+const int kMaxOutOfPlace = 1 << 30;                                       // larger blocks are compressed in place (libbsc.cpp:124-210)
 
 struct Options {
     int block_bytes = 25 << 20, sorter = 1, coder = 1, slots = 96;
@@ -77,7 +81,7 @@ const char *error_text(int code)
 {
     switch (code) {
     case -2: return "not enough memory";
-    case -4: return "method not supported by this build (see DESIGN.md 1: ST decoding, gated coders and LZP)";
+    case -4: return "method not supported by this build (see DESIGN.md 1: -m3..8 above -b1024)";
     case -5: return "unexpected end of block";
     case -6: return "the compressed data is corrupted";
     case -7: return "general GPU failure";
@@ -106,15 +110,19 @@ void put_record(unsigned char *rec, long long offset, int recordSize, int contex
 
 // Blocks in flight per GPU, bounded by its free memory: a context holds the staged block + the coder stage (~15 n + 64 MB); the sort
 // slabs (~58 n each for BWT; three are reserved here, the library makes up to six while memory lasts) are shared by all of them.  At -b1024 that is one or two blocks, at -b25 the full -j.
+// A block above 1 GiB takes the library's bounded in-place path: bscb200_inplace_bytes each (18 n + 256 MiB, in either direction), no slabs;
+// at -b2047 an 80 GB card runs one at a time.
 int fit_slots(const Options &opt, int want)
 {
     int slots = want;
+    const bool big = opt.block_bytes > kMaxOutOfPlace;
     for (int dev : opt.devices) {
         if (bscb200_set_device(dev) != 0) die("cannot select GPU");
         const long long fr = bscb200_device_free_bytes();
         if (fr < 0) continue;
-        const long long per = 2LL * opt.block_bytes + bscb200_workspace_bytes(opt.block_bytes, opt.sorter) + (64LL << 20);
-        const long long avail = fr - fr / 10 - 3 * bscb200_scratch_bytes(opt.block_bytes, opt.sorter);
+        const long long per = big ? bscb200_inplace_bytes(opt.block_bytes, 1, 1)
+                                  : 2LL * opt.block_bytes + bscb200_workspace_bytes(opt.block_bytes, opt.sorter) + (64LL << 20);
+        const long long avail = fr - fr / 10 - (big ? 0 : 3 * bscb200_scratch_bytes(opt.block_bytes, opt.sorter));
         const int fit = per > 0 ? (int)std::max(1LL, avail / per) : want;
         slots = std::min(slots, fit);
     }
@@ -159,7 +167,7 @@ int compress_file(const char *in_name, const char *out_name, Options opt)
     opt.slots = (W + (int)opt.devices.size() - 1) / (int)opt.devices.size();
 
     run_workers(opt, [&](int) {
-        std::vector<unsigned char> in((size_t)opt.block_bytes), out;
+        std::vector<unsigned char> in, out;
         for (;;) {
             int b;
             {   // bounded look-ahead: a worker may run at most 2 W blocks ahead of the writer
@@ -170,10 +178,22 @@ int compress_file(const char *in_name, const char *out_name, Options opt)
             }
             const long long off = (long long)b * opt.block_bytes;
             const int n = (int)std::min<long long>(opt.block_bytes, size - off);
-            pread_all(fin, in.data(), (size_t)n, (off_t)off, in_name);
             out.assign((size_t)n + LIBBSC_HEADER_SIZE + kRecordBytes, 0);
             put_record(out.data(), off, 1, kContextsFollowing);
-            const int r = bsc_compress(in.data(), out.data() + kRecordBytes, n, opt.lzp_hash, opt.lzp_min, opt.sorter, opt.coder, kFeatures);   // stores incompressible blocks itself
+            unsigned char *blk = out.data() + kRecordBytes;
+            int r;
+            if (n <= kMaxOutOfPlace) {
+                if (in.size() < (size_t)n) in.resize((size_t)n);
+                pread_all(fin, in.data(), (size_t)n, (off_t)off, in_name);
+                r = bsc_compress(in.data(), blk, n, opt.lzp_hash, opt.lzp_min, opt.sorter, opt.coder, kFeatures);   // stores incompressible blocks itself
+            } else {                                                              // in place, as bsc.cpp:354-376 compresses every block
+                pread_all(fin, blk, (size_t)n, (off_t)off, in_name);
+                r = bsc_compress(blk, blk, n, opt.lzp_hash, opt.lzp_min, opt.sorter, opt.coder, kFeatures);
+                if (r == LIBBSC_NOT_COMPRESSIBLE) {                              // the reference's library destroys the buffer here (this one does not)
+                    pread_all(fin, blk, (size_t)n, (off_t)off, in_name);
+                    r = bsc_store(blk, blk, n, kFeatures);
+                }
+            }
             if (r < LIBBSC_NO_ERROR) die("\nCompression failed: %s", error_text(r));
             out.resize((size_t)r + kRecordBytes);
             std::unique_lock<std::mutex> lk(mu);
@@ -273,9 +293,10 @@ void usage()
     fprintf(stdout,
             "bsc_b200 -- libbsc-compatible block-sorting compressor on NVIDIA H100 GPUs (bsc1 container)\n\n"
             "Usage: bsc_b200 <e|d> inputfile outputfile <options>\n"
-            "  -b<size>  block size in MiB, default -b25 (1..1024)\n"
-            "  -m<algo>  block sorter: -m0 Burrows-Wheeler transform (default), -m3..-m8 sort transform of order n (encode only)\n"
-            "  -e<algo>  entropy coder: -e1 static QLFC (default), -e0 fast, -e2 adaptive (experimental, see DESIGN.md)\n"
+            "  -b<size>  block size in MiB, default -b25 (1..2047; blocks above 1024 are compressed in place in at most 18 n + 256 MiB of HBM\n"
+            "            each, -m0 only)\n"
+            "  -m<algo>  block sorter: -m0 Burrows-Wheeler transform (default), -m3..-m8 sort transform of order n\n"
+            "  -e<algo>  entropy coder: -e1 static QLFC (default), -e0 fast, -e2 adaptive\n"
             "  -l        LZP preprocessing on (host stage; -H<10..28> hash bits, -M<4..255> minimum match; bsc's defaults 15 / 128)\n"
             "  -g<list>  GPUs to use, e.g. -g0,1,2,3 (default: all visible)\n"
             "  -j<n>     blocks in flight per GPU, default -j96, fewer when HBM is short (8 coder streams per block, up to five per SM)\n"
@@ -294,7 +315,7 @@ int main(int argc, char **argv)
         if (a[0] != '-' || !a[1]) usage();
         const int v = atoi(a + 2);
         switch (a[1]) {
-        case 'b': if (v < 1 || v > 1024) usage(); opt.block_bytes = v == 1024 ? 1073741824 : v << 20; break;
+        case 'b': if (v < 1 || v > 2047) usage(); opt.block_bytes = v << 20; break;            // bsc.cpp:761: up to 2047 MiB
         case 'm': if (v != 0 && (v < 3 || v > 8)) usage(); opt.sorter = v == 0 ? 1 : v; break;
         case 'e': if (v < 0 || v > 2) usage(); opt.coder = v == 0 ? 3 : v; break;
         case 'j': if (v < 1 || v > 64) usage(); opt.slots = v; break;

@@ -272,6 +272,7 @@ int store_dev(Ctx *ctx, const u8 *d_in, int n, u8 *d_out, u32 adler_data)
 // is lz->adler_orig; the header describes the original block, and a block that does not shrink is reported as LIBBSC_NOT_COMPRESSIBLE
 // (the caller stores the ORIGINAL data, libbsc.cpp:315-318).
 struct LzpInfo { int orig_n; u32 adler_orig; int mode_bits; };
+int finish_dev(Ctx *ctx, u8 *d_out, int result, unsigned char num_indexes, const int *indexes, int orig_n, int mode, int index, u32 adler_data);
 
 int compress_dev(Ctx *ctx, const u8 *d_in, int n, u8 *d_out, int blockSorter, int coder, int features, bool inplace_rules, const LzpInfo *lz = nullptr)
 {
@@ -302,6 +303,12 @@ int compress_dev(Ctx *ctx, const u8 *d_in, int n, u8 *d_out, int blockSorter, in
         if (inplace_rules || lz) return LIBBSC_NOT_COMPRESSIBLE;         // libbsc.cpp:188-191
         return store_dev(ctx, d_in, n, d_out, adler_data);               // libbsc.cpp:315-318
     }
+    return finish_dev(ctx, d_out, result, num_indexes, indexes, orig_n, mode, index, adler_data);
+}
+
+// The secondary indexes and the header of a compressed block whose coder output (`result` bytes) is at d_out + 28.
+int finish_dev(Ctx *ctx, u8 *d_out, int result, unsigned char num_indexes, const int *indexes, int orig_n, int mode, int index, u32 adler_data)
+{
     unsigned char *tail = (unsigned char *)(ctx->h_mail + 96);            // pinned, <= 4*255+1 bytes needs care: num_indexes <= 15 here
     memcpy(tail, indexes, 4 * (size_t)num_indexes);
     tail[4 * num_indexes] = num_indexes;
@@ -373,6 +380,84 @@ int decompress_dev(Ctx *ctx, const unsigned char *h, const u8 *d_block, int inpu
     if (lzp) { *lz_out = lzSize; return LIBBSC_NO_ERROR; }
     if (lzSize != dataSize) return LIBBSC_DATA_CORRUPT;
     return adler_data == stage_adler32(ctx, d_out, dataSize) ? LIBBSC_NO_ERROR : LIBBSC_DATA_CORRUPT;
+}
+
+// ---------------------------------------------------------------------------------------------
+// blocks above 1 GiB: in-place bsc_compress, and bsc_decompress of such blocks
+// ---------------------------------------------------------------------------------------------
+// On the pooled path a block of n bytes holds about 31 n of HBM: the staged block, its working copy, the output and the coder stage in
+// the context, and a 16.5 n sort slab that the pool keeps after the call.  A block above 1 GiB instead runs on a context made for the
+// call and destroyed after it, in ONE allocation: the block, sorted in place (an in-place call may destroy its input, libbsc.cpp:160),
+// and a region that first holds the batched forward BWT (16 n + 32 B) and then the coder stage with its output (about 13 n + 64 MB).
+// The caller's buffer is written only once the block is done.  Only the BWT has a bounded sorter: the forward ST needs about 30 n and
+// the inverse ST about 41 n (need_st_encode, need_st_decode), so ST3..ST8 stay at 1 GiB.
+// The arena is 17.5 n + 128 MiB: the batched sort at batches of about n / 64 entries (16.5 n) or the coder stage with its output
+// (at most 13 n + 64 MB) after the block.  The bound adds n / 2 + 128 MiB for what lies outside the arena: the context, the coder
+// tables, kernel images loaded on first use and the driver's own transient allocations (about 0.55 GB measured at the largest n).
+constexpr int LARGE_N = 1073741824;                  // blocks above this take the path below
+constexpr size_t LARGE_FIXED = 256u << 20;
+size_t large_bound(size_t n) { return 18 * n + LARGE_FIXED; }
+size_t large_arena(size_t n) { return 17 * n + n / 2 + LARGE_FIXED / 2; }
+
+// run `body(ctx)` on a context of its own, destroyed afterwards so that none of its HBM outlives the call
+template <class F> int with_own_ctx(F body)
+{
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess) { cudaGetLastError(); return LIBBSC_GPU_NOT_SUPPORTED; }
+    Ctx *c = nullptr;
+    try { c = ctx_new(dev, nullptr, true); }
+    catch (const CudaFail &f) { return map_failure(f); }
+    catch (...) { cudaGetLastError(); return LIBBSC_GPU_ERROR; }
+    int r;
+    try { r = body(c); }
+    catch (const CudaFail &f) { r = map_failure(f); }
+    catch (const std::bad_alloc &) { r = LIBBSC_NOT_ENOUGH_MEMORY; }
+    catch (...) { r = LIBBSC_GPU_ERROR; }
+    cudaStreamSynchronize(c->stream); cudaGetLastError();
+    { std::lock_guard<std::mutex> lk(g_pool_mutex); g_launches_retired += c->kernels_launched; }
+    ctx_delete(c);
+    return r;
+}
+
+// In-place bsc_compress of a block of n > 1 GiB bytes with the BWT sorter (libbsc.cpp:124-210).
+int compress_large(unsigned char *data, int n, int lzpHashSize, int lzpMinLen, int coder, int features)
+{
+    size_t fr = 0, total = 0;
+    if (cudaMemGetInfo(&fr, &total) != cudaSuccess) { cudaGetLastError(); return LIBBSC_GPU_NOT_SUPPORTED; }
+    if (fr < large_bound((size_t)n)) return LIBBSC_GPU_NOT_ENOUGH_MEMORY;
+
+    int m = n, mode_bits = 0; u32 adler_orig = 0;          // m: bytes that go through the sort and the coder
+    unsigned char *lzbuf = nullptr;
+    if (lzpMinLen != 0) {                                   // libbsc.cpp:139-154: LZP on the host, not in place
+        lzbuf = (unsigned char *)bsc_malloc((size_t)n + 64);
+        if (!lzbuf) return LIBBSC_NOT_ENOUGH_MEMORY;
+        const int lzSize = lzp_host::compress(data, lzbuf, n, lzpHashSize, lzpMinLen, (features & LIBBSC_FEATURE_MULTITHREADING) != 0);
+        if (lzSize >= 0) { m = lzSize; mode_bits = (lzpMinLen << 8) | (lzpHashSize << 16); adler_orig = host_adler32(data, (size_t)n); }
+        else { bsc_free(lzbuf); lzbuf = nullptr; }         // LZP did not shrink the block: continue without it (mode &= 0xff)
+    }
+    const unsigned char *src = lzbuf ? lzbuf : data;
+    const int r = with_own_ctx([&](Ctx *ctx) {
+        Arena &A = ctx->arena;
+        A.reserve(large_arena((size_t)n));
+        u8 *d_blk = A.get<u8>((size_t)m + 64);
+        CUDA_TRY(cudaMemcpyAsync(d_blk, src, (size_t)m, cudaMemcpyHostToDevice, ctx->stream));
+        const u32 adler_data = lzbuf ? adler_orig : stage_adler32(ctx, d_blk, m);
+        // the sort may use the whole region after the block (less a margin for the arena's rounding): batches of about n / 64 entries
+        const u32 B = bwt_batch_entries((u32)m, (long long)(A.cap - A.used) - (16ll << 20));
+        int indexes[256]; unsigned char num_indexes = 0;
+        const int index = stage_bwt_encode_batched(ctx, d_blk, m, &num_indexes, indexes, B);
+        if (index < 0) return index;
+        u8 *d_out = A.get<u8>((size_t)m + 4096) + 4;       // payload (offset 28) lands 16-byte aligned
+        const int result = stage_coder_compress(ctx, d_blk, d_out + LIBBSC_HEADER_SIZE, m, coder, features);
+        if (result == LIBBSC_NOT_SUPPORTED) return result;
+        if (result < 0 || result + 1 + 4 * num_indexes >= n) return LIBBSC_NOT_COMPRESSIBLE;     // libbsc.cpp:188-191
+        const int size = finish_dev(ctx, d_out, result, num_indexes, indexes, n, 1 | (coder << 5) | mode_bits, index, adler_data);
+        CUDA_TRY(cudaMemcpyAsync(data, d_out, (size_t)size, cudaMemcpyDeviceToHost, ctx->stream));
+        ctx->sync();
+        return size;
+    });
+    if (lzbuf) bsc_free(lzbuf);
+    return r;
 }
 
 }  // namespace
@@ -453,7 +538,7 @@ int bsc_compress(const unsigned char *input, unsigned char *output, int n, int l
     }
     const bool inplace = (input == output);
     if (n < 0 || n > (inplace ? 2146435072 : 1073741824)) return LIBBSC_BAD_PARAMETER;
-    if (n > 1073741824) return LIBBSC_NOT_SUPPORTED;
+    if (n > LARGE_N) return blockSorter == 1 ? compress_large(output, n, lzpHashSize, lzpMinLen, coder, features) : LIBBSC_NOT_SUPPORTED;
     if (n <= LIBBSC_HEADER_SIZE) return bsc_store(input, output, n, features);
     if (lzpMinLen != 0) {                                   // libbsc.cpp:264-276
         unsigned char *lzbuf = (unsigned char *)bsc_malloc((size_t)n + 64);
@@ -494,7 +579,8 @@ int bsc_decompress(const unsigned char *input, int inputSize, unsigned char *out
     if (info != LIBBSC_NO_ERROR) return info;
     if (inputSize < blockSize || outputSize < dataSize) return LIBBSC_UNEXPECTED_EOB;
     unsigned char h[LIBBSC_HEADER_SIZE]; memcpy(h, input, LIBBSC_HEADER_SIZE);
-    return with_ctx([&](Ctx *ctx) {
+    // Above 1 GiB: about 14 n + 64 MB (large_bound holds it), on a context of its own that does not keep it after the call.
+    auto body = [&](Ctx *ctx) {
         ctx->arena.reserve((size_t)blockSize + (size_t)dataSize + 8192 + need_coder((size_t)dataSize));      // coder stage, then the inverse BWT in the same space
         u8 *d_blk = ctx->arena.get<u8>((size_t)blockSize + 128) + 4;
         u8 *d_out = ctx->arena.get<u8>((size_t)dataSize + 128);
@@ -514,7 +600,8 @@ int bsc_decompress(const unsigned char *input, int inputSize, unsigned char *out
         }
         if (r == LIBBSC_NO_ERROR && dataSize > 0) { CUDA_TRY(cudaMemcpyAsync(output, d_out, (size_t)dataSize, cudaMemcpyDeviceToHost, ctx->stream)); ctx->sync(); }
         return r;
-    });
+    };
+    return dataSize > LARGE_N ? with_own_ctx(body) : with_ctx(body);
 }
 
 int bsc_bwt_encode(unsigned char *T, int n, unsigned char *num_indexes, int *indexes, int features)
@@ -727,6 +814,13 @@ long long bscb200_scratch_bytes(int n, int blockSorter)     /* size of one share
     size_t s = (blockSorter == 1 ? need_bwt_encode((size_t)n) : need_st_encode((size_t)n));
     size_t d = blockSorter == 1 ? 0 : need_st_decode((size_t)n);
     return (long long)(s > d ? s : d);
+}
+// HBM that an in-place bsc_compress of a block above 1 GiB, or bsc_decompress of one, takes at most: 18 n + 256 MiB (large_bound)
+long long bscb200_inplace_bytes(int n, int blockSorter, int coder)
+{
+    if (n < 0 || n > 2146435072 || !sorter_valid(blockSorter) || coder < 1 || coder > 3) return LIBBSC_BAD_PARAMETER;
+    if (blockSorter != 1) return LIBBSC_NOT_SUPPORTED;      // no bounded sort transform
+    return (long long)large_bound((size_t)n);
 }
 // host-only: the inverse LZP stage by itself (what bsc_decompress runs after the GPU stages), for CPU tests against the reference
 int bscb200_lzp_decompress_host(const unsigned char *input, int n, unsigned char *output, int outputCapacity, int lzpHashSize, int lzpMinLen)
