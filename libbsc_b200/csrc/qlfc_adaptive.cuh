@@ -10,7 +10,8 @@
 // So a decision costs about three times the instructions of a static one, and the working set grows by 1896 mixers x 48 B
 // and 16 KB of tables: counter file in the two-streams-per-SM layout of qlfc_decoder6.cuh (110 KB) + 107 KB = 215 KB,
 // one stream per SM.  Both directions are one lock-step warp per stream (decision by decision).
-// STATUS: bit-exact in host emulation; NOT yet run on a GPU -> behind BSCB200_ENABLE_ADAPTIVE=1 (LIBBSC_NOT_SUPPORTED otherwise).
+// STATUS: bit-exact in host emulation and on the GPU (tests/test_gpu_other_coders.py, tests/test_gpu_pipeline.py); enabled
+// without any switch (coder_gate in qlfc.cu).
 #pragma once
 
 typedef QLayout<4, 2, 10> ALY;                                  // counter file (qlfc_decoder6.cuh)

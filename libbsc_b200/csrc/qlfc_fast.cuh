@@ -11,8 +11,8 @@
 // write-back cache in front of the rare remainder (rank exponents 6-7, run exponents > 5; 768 KB in HBM per stream).
 // Both directions are one lock-step warp per stream for now: a decision is one shared-memory load, one shift-update
 // and one branch-free range-coder step.
-// STATUS: bit-exact in host emulation; NOT yet run on a GPU (no GPU budget was left in round 1), so the product
-// dispatch keeps coder 3 behind BSCB200_ENABLE_FAST=1 and answers LIBBSC_NOT_SUPPORTED otherwise.
+// STATUS: bit-exact in host emulation and on the GPU (tests/test_gpu_other_coders.py, tests/test_gpu_pipeline.py); enabled
+// without any switch (coder_gate in qlfc.cu).
 #pragma once
 
 constexpr u32 QF_ROW = 62, QF_MAXE = 5;                        // compact mantissa row: exponents 1..5 at offsets 2^e-2 .. 2^(e+1)-3
