@@ -58,8 +58,10 @@ int bsc_init_full(int features, void *(*malloc_fn)(size_t), void *(*zero_malloc_
  * n > 1 GiB is LIBBSC_BAD_PARAMETER as in the reference.  An in-place block above 1 GiB is sorted in place with the batched forward
  * BWT on a context of its own, in at most bscb200_inplace_bytes() = 18 n + 256 MiB of HBM, all of it freed when the call returns;
  * LIBBSC_GPU_NOT_ENOUGH_MEMORY (nothing written) when the device has less free.  The caller's buffer is written only on success.
- * Above 1 GiB the sort transforms (blockSorter 3..8) return LIBBSC_NOT_SUPPORTED: they need about 30 n to encode and 41 n to decode
- * and have no bounded variant. */
+ * Above 1 GiB bsc_compress with the sort transforms (blockSorter 3..8) returns LIBBSC_NOT_SUPPORTED: the forward ST needs about 30 n
+ * and has no bounded variant.  bsc_decompress reads every block the reference writes, up to 2146435072 bytes with every sorter: a block
+ * above 1 GiB runs on a context of its own, in at most bscb200_decompress_bytes() of HBM (18 n + 256 MiB for the BWT, 26.5 n + 256 MiB
+ * for ST3..ST8), all of it freed when the call returns; LIBBSC_GPU_NOT_ENOUGH_MEMORY when the device has less free. */
 int bsc_compress(const unsigned char *input, unsigned char *output, int n, int lzpHashSize, int lzpMinLen, int blockSorter, int coder, int features);
 /* libbsc/libbsc.h:128 ; libbsc.cpp:68-81 */
 int bsc_store(const unsigned char *input, unsigned char *output, int n, int features);
@@ -133,6 +135,10 @@ long long          bscb200_scratch_bytes(int n, int blockSorter);  /* one device
  * n = 2146435072), none of it kept after the call.  Same for the three coders and with LZP.  Blocks of at most 1 GiB take the pooled path
  * instead (bscb200_workspace_bytes + bscb200_scratch_bytes).  blockSorter 3..8: LIBBSC_NOT_SUPPORTED; bad arguments: LIBBSC_BAD_PARAMETER. */
 long long          bscb200_inplace_bytes(int n, int blockSorter, int coder);
+/* HBM that bsc_decompress of a block with data size n and this blockSorter takes at most.  Above 1 GiB: 18 n + 256 MiB for the BWT
+ * (= bscb200_inplace_bytes(n, 1, 1)) and 26.5 n + 256 MiB for ST3..ST8 (about 57.2 GB at n = 2146435072), none of it kept after the call.
+ * Up to 1 GiB: the pooled cost, bscb200_workspace_bytes + bscb200_scratch_bytes.  Bad arguments: LIBBSC_BAD_PARAMETER. */
+long long          bscb200_decompress_bytes(int n, int blockSorter);
 unsigned long long bscb200_ctx_kernel_launches(void *ctx);
 unsigned long long bscb200_total_kernel_launches(void);
 /* per-kernel CUDA-event timing of everything launched through ctx (bench.py's roofline leg) */

@@ -48,6 +48,7 @@ static long long bscb200_device_free_bytes(void) { return -1; }
 static long long bscb200_workspace_bytes(int, int) { return 0; }
 static long long bscb200_scratch_bytes(int, int) { return 0; }
 static long long bscb200_inplace_bytes(int, int, int) { return 0; }
+static long long bscb200_decompress_bytes(int, int) { return 0; }
 static void bscb200_release_pools(void) {}
 static int bscb200_set_device(int) { return 0; }
 #define LIBBSC_HEADER_SIZE 28
@@ -110,9 +111,10 @@ void put_record(unsigned char *rec, long long offset, int recordSize, int contex
 
 // Blocks in flight per GPU, bounded by its free memory: a context holds the staged block + the coder stage (~15 n + 64 MB); the sort
 // slabs (~58 n each for BWT; three are reserved here, the library makes up to six while memory lasts) are shared by all of them.  At -b1024 that is one or two blocks, at -b25 the full -j.
-// A block above 1 GiB takes the library's bounded in-place path: bscb200_inplace_bytes each (18 n + 256 MiB, in either direction), no slabs;
-// at -b2047 an 80 GB card runs one at a time.
-int fit_slots(const Options &opt, int want)
+// A block above 1 GiB takes the library's bounded path on a context of its own, no slabs: bscb200_inplace_bytes to compress (18 n + 256 MiB,
+// BWT only), bscb200_decompress_bytes of the block's sorter to decompress (the same for the BWT, 26.5 n + 256 MiB for ST3..ST8); at -b2047 an
+// 80 GB card runs one at a time.
+int fit_slots(const Options &opt, int want, bool decode = false)
 {
     int slots = want;
     const bool big = opt.block_bytes > kMaxOutOfPlace;
@@ -120,7 +122,7 @@ int fit_slots(const Options &opt, int want)
         if (bscb200_set_device(dev) != 0) die("cannot select GPU");
         const long long fr = bscb200_device_free_bytes();
         if (fr < 0) continue;
-        const long long per = big ? bscb200_inplace_bytes(opt.block_bytes, 1, 1)
+        const long long per = big ? (decode ? bscb200_decompress_bytes(opt.block_bytes, opt.sorter) : bscb200_inplace_bytes(opt.block_bytes, 1, 1))
                                   : 2LL * opt.block_bytes + bscb200_workspace_bytes(opt.block_bytes, opt.sorter) + (64LL << 20);
         const long long avail = fr - fr / 10 - (big ? 0 : 3 * bscb200_scratch_bytes(opt.block_bytes, opt.sorter));
         const int fit = per > 0 ? (int)std::max(1LL, avail / per) : want;
@@ -215,7 +217,7 @@ int compress_file(const char *in_name, const char *out_name, Options opt)
 }
 
 // ------------------------------------------------------------------------------------------------------------------
-struct BlockRef { long long file_pos, out_offset; int block_size, data_size, record_size, contexts; };
+struct BlockRef { long long file_pos, out_offset; int block_size, data_size, record_size, contexts, sorter; };
 
 // inverses of the reference's host-side filters, applied after the block is decoded (bsc.cpp:614-647):
 // reversed contexts (preprocessing.cpp:41-66) and record reordering (preprocessing.cpp:123-178: column-major back to records)
@@ -257,6 +259,7 @@ int decompress_file(const char *in_name, const char *out_name, Options opt)
         BlockRef r; r.file_pos = pos + kRecordBytes; r.out_offset = off; r.record_size = recordSize; r.contexts = contexts;
         if (bsc_block_info(rec + kRecordBytes, LIBBSC_HEADER_SIZE, &r.block_size, &r.data_size, kFeatures) != LIBBSC_NO_ERROR) die("This is not bsc archive or invalid compression method!");
         if (r.file_pos + r.block_size > size) die("Unexpected end of file: %s!", in_name);
+        r.sorter = rec[kRecordBytes + 8] & 0x1f;                         // header mode, bits 0..4 (0: a stored block)
         blocks.push_back(r);
         pos = r.file_pos + r.block_size;
     }
@@ -264,7 +267,13 @@ int decompress_file(const char *in_name, const char *out_name, Options opt)
     const int nBlocks = (int)blocks.size();
     const double t0 = now();
     std::mutex mu; int next = 0; long long out_size = 0;
-    { int big = 0; for (const BlockRef &r : blocks) big = std::max(big, r.data_size); Options o2 = opt; o2.block_bytes = big; o2.sorter = 6; opt.slots = fit_slots(o2, opt.slots); }
+    {   // sized for the largest block, with its sorter above 1 GiB (an ST block of equal size needs more than a BWT one)
+        Options o2 = opt; o2.block_bytes = 0; o2.sorter = 1;
+        for (const BlockRef &r : blocks)
+            if (r.data_size > o2.block_bytes || (r.data_size == o2.block_bytes && r.sorter >= 3)) { o2.block_bytes = r.data_size; o2.sorter = r.sorter >= 3 ? r.sorter : 1; }
+        if (o2.block_bytes <= kMaxOutOfPlace) o2.sorter = 6;
+        opt.slots = fit_slots(o2, opt.slots, true);
+    }
     const int W = std::max(1, std::min((int)opt.devices.size() * opt.slots, nBlocks));
     opt.slots = (W + (int)opt.devices.size() - 1) / (int)opt.devices.size();
     run_workers(opt, [&](int) {
@@ -294,7 +303,7 @@ void usage()
             "bsc_b200 -- libbsc-compatible block-sorting compressor on NVIDIA H100 GPUs (bsc1 container)\n\n"
             "Usage: bsc_b200 <e|d> inputfile outputfile <options>\n"
             "  -b<size>  block size in MiB, default -b25 (1..2047; blocks above 1024 are compressed in place in at most 18 n + 256 MiB of HBM\n"
-            "            each, -m0 only)\n"
+            "            each, -m0 only: -m3..8 above 1024 decode, in at most 26.5 n + 256 MiB each, but do not encode)\n"
             "  -m<algo>  block sorter: -m0 Burrows-Wheeler transform (default), -m3..-m8 sort transform of order n\n"
             "  -e<algo>  entropy coder: -e1 static QLFC (default), -e0 fast, -e2 adaptive\n"
             "  -l        LZP preprocessing on (host stage; -H<10..28> hash bits, -M<4..255> minimum match; bsc's defaults 15 / 128)\n"

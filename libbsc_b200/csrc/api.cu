@@ -389,8 +389,8 @@ int decompress_dev(Ctx *ctx, const unsigned char *h, const u8 *d_block, int inpu
 // the context, and a 16.5 n sort slab that the pool keeps after the call.  A block above 1 GiB instead runs on a context made for the
 // call and destroyed after it, in ONE allocation: the block, sorted in place (an in-place call may destroy its input, libbsc.cpp:160),
 // and a region that first holds the batched forward BWT (16 n + 32 B) and then the coder stage with its output (about 13 n + 64 MB).
-// The caller's buffer is written only once the block is done.  Only the BWT has a bounded sorter: the forward ST needs about 30 n and
-// the inverse ST about 41 n (need_st_encode, need_st_decode), so ST3..ST8 stay at 1 GiB.
+// The caller's buffer is written only once the block is done.  Only the BWT has a bounded forward sorter: the forward ST needs about
+// 30 n (need_st_encode), so ST3..ST8 compress only up to 1 GiB.  Their inverse has a lean layout (decompress_large_st below).
 // The arena is 17.5 n + 128 MiB: the batched sort at batches of about n / 64 entries (16.5 n) or the coder stage with its output
 // (at most 13 n + 64 MB) after the block.  The bound adds n / 2 + 128 MiB for what lies outside the arena: the context, the coder
 // tables, kernel images loaded on first use and the driver's own transient allocations (about 0.55 GB measured at the largest n).
@@ -398,6 +398,13 @@ constexpr int LARGE_N = 1073741824;                  // blocks above this take t
 constexpr size_t LARGE_FIXED = 256u << 20;
 size_t large_bound(size_t n) { return 18 * n + LARGE_FIXED; }
 size_t large_arena(size_t n) { return 17 * n + n / 2 + LARGE_FIXED / 2; }
+// bsc_decompress of an ST3..ST8 block whose data size n is above 1 GiB: ONE arena holds L (n + 128) and a region of
+// st_decode_lean_bytes(n) = 25 n + 1 MiB after it.  The compressed block (at most n + 28) sits at the top end of that region while the
+// coder stage (at most 12 n + 64 MB) works below it; the inverse ST then takes the whole region in its lean layout (st_decode.cu), and
+// its output lands there too.  26 n + 1 MiB in all, the block included.  The bound adds n / 2 + 255 MiB for what lies outside the
+// arena, as large_bound does: 26.5 n + 256 MiB, 57.2 GB at n = 2146435072.
+size_t large_st_arena(size_t n) { return align_up(n + 128 + 256, 256) + align_up(st_decode_lean_bytes(n), 256); }
+size_t large_st_bound(size_t n) { return 26 * n + n / 2 + LARGE_FIXED; }
 
 // run `body(ctx)` on a context of its own, destroyed afterwards so that none of its HBM outlives the call
 template <class F> int with_own_ctx(F body)
@@ -458,6 +465,52 @@ int compress_large(unsigned char *data, int n, int lzpHashSize, int lzpMinLen, i
     });
     if (lzbuf) bsc_free(lzbuf);
     return r;
+}
+
+// libbsc.cpp:599-613: undo the LZP stage of a block (header h) on the host, from the lzSize-byte LZP stream at d_lz
+int undo_lzp_host(Ctx *ctx, const unsigned char *h, const u8 *d_lz, int lzSize, unsigned char *output, int dataSize)
+{
+    const int mode = (int)get32(h + 8);
+    unsigned char *lz = (unsigned char *)bsc_malloc((size_t)lzSize + 1);
+    if (!lz) return LIBBSC_NOT_ENOUGH_MEMORY;
+    if (lzSize > 0) { CUDA_TRY(cudaMemcpyAsync(lz, d_lz, (size_t)lzSize, cudaMemcpyDeviceToHost, ctx->stream)); ctx->sync(); }
+    int r = lzp_host::decompress(lz, lzSize, output, dataSize, (mode >> 16) & 0xff, (mode >> 8) & 0xff);
+    bsc_free(lz);
+    if (r < 0) return r;
+    return (r == dataSize && get32(h + 16) == host_adler32(output, (size_t)dataSize)) ? LIBBSC_NO_ERROR : LIBBSC_DATA_CORRUPT;
+}
+
+// bsc_decompress of a block with block sorter 3..8 whose data size is above 1 GiB (large_st_arena above).  The caller checked the header
+// (block_info_host) and the sizes.  Without LZP the caller's buffer is written only on success.
+int decompress_large_st(const unsigned char *input, const unsigned char *h, int blockSize, int dataSize, unsigned char *output, int features)
+{
+    size_t fr = 0, total = 0;
+    if (cudaMemGetInfo(&fr, &total) != cudaSuccess) { cudaGetLastError(); return LIBBSC_GPU_NOT_SUPPORTED; }
+    if (fr < large_st_bound((size_t)dataSize)) return LIBBSC_GPU_NOT_ENOUGH_MEMORY;
+    return with_own_ctx([&](Ctx *ctx) {
+        Arena &A = ctx->arena;
+        A.reserve(large_st_arena((size_t)dataSize));
+        u8 *d_L = A.get<u8>((size_t)dataSize + 128);
+        const size_t full = A.cap, blk = align_up((size_t)blockSize + 128, 256);
+        u8 *d_blk = A.base + full - blk + 4;                 // the top end of the region; payload (offset 28) lands 16-byte aligned
+        CUDA_TRY(cudaMemcpyAsync(d_blk, input, (size_t)blockSize, cudaMemcpyHostToDevice, ctx->stream));
+        CUDA_TRY(cudaMemsetAsync(d_blk + blockSize, 0, 64, ctx->stream));
+        const int payload = blockSize - LIBBSC_HEADER_SIZE, mode = (int)get32(h + 8), index = (int)get32(h + 12);
+        if (payload < 1) return LIBBSC_DATA_CORRUPT;
+        if (get32(h + 20) != stage_adler32(ctx, d_blk + LIBBSC_HEADER_SIZE, payload)) return LIBBSC_DATA_CORRUPT;
+        A.cap = full - blk;                                  // the coder stage stays below the block
+        const int lzSize = stage_coder_decompress(ctx, d_blk + LIBBSC_HEADER_SIZE, payload, d_L, dataSize, (mode >> 5) & 7, features);
+        A.cap = full;
+        if (lzSize < 0) return lzSize;
+        u8 *d_T = nullptr;                                   // the block is dead: the inverse ST takes the whole region after L
+        const int r = stage_st_decode_lean(ctx, d_L, lzSize, mode & 0x1f, index, &d_T);
+        if (r < 0) return r;
+        if (mode != (mode & 0xff)) return undo_lzp_host(ctx, h, d_T, lzSize, output, dataSize);
+        if (lzSize != dataSize || get32(h + 16) != stage_adler32(ctx, d_T, dataSize)) return LIBBSC_DATA_CORRUPT;
+        CUDA_TRY(cudaMemcpyAsync(output, d_T, (size_t)dataSize, cudaMemcpyDeviceToHost, ctx->stream));
+        ctx->sync();
+        return LIBBSC_NO_ERROR;
+    });
 }
 
 }  // namespace
@@ -579,7 +632,8 @@ int bsc_decompress(const unsigned char *input, int inputSize, unsigned char *out
     if (info != LIBBSC_NO_ERROR) return info;
     if (inputSize < blockSize || outputSize < dataSize) return LIBBSC_UNEXPECTED_EOB;
     unsigned char h[LIBBSC_HEADER_SIZE]; memcpy(h, input, LIBBSC_HEADER_SIZE);
-    // Above 1 GiB: about 14 n + 64 MB (large_bound holds it), on a context of its own that does not keep it after the call.
+    if (dataSize > LARGE_N && (get32(h + 8) & 0x1f) >= 3) return decompress_large_st(input, h, blockSize, dataSize, output, features);
+    // Above 1 GiB (BWT and stored blocks): about 14 n + 64 MB (large_bound holds it), on a context of its own that does not keep it after the call.
     auto body = [&](Ctx *ctx) {
         ctx->arena.reserve((size_t)blockSize + (size_t)dataSize + 8192 + need_coder((size_t)dataSize));      // coder stage, then the inverse BWT in the same space
         u8 *d_blk = ctx->arena.get<u8>((size_t)blockSize + 128) + 4;
@@ -588,16 +642,7 @@ int bsc_decompress(const unsigned char *input, int inputSize, unsigned char *out
         CUDA_TRY(cudaMemsetAsync(d_blk + blockSize, 0, 64, ctx->stream));
         int lzSize = -1;
         int r = decompress_dev(ctx, h, d_blk, blockSize, d_out, dataSize, features, &lzSize);
-        if (r == LIBBSC_NO_ERROR && lzSize >= 0) {                       // libbsc.cpp:599-613: undo the LZP stage on the host
-            const int mode = (int)get32(h + 8);
-            unsigned char *lz = (unsigned char *)bsc_malloc((size_t)lzSize + 1);
-            if (!lz) return LIBBSC_NOT_ENOUGH_MEMORY;
-            if (lzSize > 0) { CUDA_TRY(cudaMemcpyAsync(lz, d_out, (size_t)lzSize, cudaMemcpyDeviceToHost, ctx->stream)); ctx->sync(); }
-            r = lzp_host::decompress(lz, lzSize, output, dataSize, (mode >> 16) & 0xff, (mode >> 8) & 0xff);
-            bsc_free(lz);
-            if (r < 0) return r;
-            return (r == dataSize && get32(h + 16) == host_adler32(output, (size_t)dataSize)) ? LIBBSC_NO_ERROR : LIBBSC_DATA_CORRUPT;
-        }
+        if (r == LIBBSC_NO_ERROR && lzSize >= 0) return undo_lzp_host(ctx, h, d_out, lzSize, output, dataSize);
         if (r == LIBBSC_NO_ERROR && dataSize > 0) { CUDA_TRY(cudaMemcpyAsync(output, d_out, (size_t)dataSize, cudaMemcpyDeviceToHost, ctx->stream)); ctx->sync(); }
         return r;
     };
@@ -821,6 +866,14 @@ long long bscb200_inplace_bytes(int n, int blockSorter, int coder)
     if (n < 0 || n > 2146435072 || !sorter_valid(blockSorter) || coder < 1 || coder > 3) return LIBBSC_BAD_PARAMETER;
     if (blockSorter != 1) return LIBBSC_NOT_SUPPORTED;      // no bounded sort transform
     return (long long)large_bound((size_t)n);
+}
+// HBM that bsc_decompress of a block with data size n takes at most: above 1 GiB the bound of its own context (large_bound for the BWT,
+// large_st_bound for ST3..ST8), else the pooled cost, one context's workspace and one shared sort slab
+long long bscb200_decompress_bytes(int n, int blockSorter)
+{
+    if (n < 0 || n > 2146435072 || !sorter_valid(blockSorter)) return LIBBSC_BAD_PARAMETER;
+    if (n > LARGE_N) return (long long)(blockSorter == 1 ? large_bound((size_t)n) : large_st_bound((size_t)n));
+    return bscb200_workspace_bytes(n, blockSorter) + bscb200_scratch_bytes(n, blockSorter);
 }
 // host-only: the inverse LZP stage by itself (what bsc_decompress runs after the GPU stages), for CPU tests against the reference
 int bscb200_lzp_decompress_host(const unsigned char *input, int n, unsigned char *output, int outputCapacity, int lzpHashSize, int lzpMinLen)

@@ -20,6 +20,11 @@ int stage_bwt_decode(Ctx *ctx, u8 *d_T, int n, int index);
 int stage_st_encode(Ctx *ctx, u8 *d_T, int n, int k);
 // Inverse sort transform in place (bsc_st_decode, st.cpp:1491; k = 3..8, index = row of rotation 0).
 int stage_st_decode(Ctx *ctx, u8 *d_T, int n, int k, int index);
+// The same inverse in the lean layout of the blocks above 1 GiB (st_decode.cu): L is read at d_L, which needs n + 64 writable bytes, and
+// the stage takes st_decode_lean_bytes(n) from ctx->arena and keeps it.  The result lands there, at *d_result (d_L itself for n <= 1).
+// LIBBSC_DATA_CORRUPT when the lists do not tile the text; the stage never writes outside its region on any input.
+int stage_st_decode_lean(Ctx *ctx, u8 *d_L, int n, int k, int index, u8 **d_result);
+size_t st_decode_lean_bytes(size_t n);
 // Coder container (bsc_coder_compress, coder.cpp:244).  d_out must hold n + 4096 bytes.
 // bare_out_size >= 0: one QLFC stream without the container (bsc_qlfc_*_encode_block, qlfc.h:55-77), output capacity bare_out_size.
 int stage_coder_compress(Ctx *ctx, const u8 *d_in, u8 *d_out, int n, int coder, int features, int bare_out_size = -1);
