@@ -395,6 +395,19 @@ int decompress_dev(Ctx *ctx, const unsigned char *h, const u8 *d_block, int inpu
 // (at most 13 n + 64 MB) after the block.  The bound adds n / 2 + 128 MiB for what lies outside the arena: the context, the coder
 // tables, kernel images loaded on first use and the driver's own transient allocations (about 0.55 GB measured at the largest n).
 constexpr int LARGE_N = 1073741824;                  // blocks above this take the path below
+// Where bsc_compress (in place) and bsc_decompress route: LARGE_N, or BSCB200_LARGE_N=<bytes> (read once per process) when it lies in
+// 0..LARGE_N.  The switch is for tests only: it lets blocks of a few bytes up take the paths below, which blocks above 1 GiB take in
+// production.  The argument limits, the HBM bounds and the CLI stay keyed on LARGE_N itself.
+int large_route_n()
+{
+    static const int v = [] {
+        const char *e = getenv("BSCB200_LARGE_N");
+        char *end = nullptr;
+        const long long t = e ? strtoll(e, &end, 10) : -1;
+        return (e && end != e && *end == '\0' && t >= 0 && t <= LARGE_N) ? (int)t : LARGE_N;
+    }();
+    return v;
+}
 constexpr size_t LARGE_FIXED = 256u << 20;
 size_t large_bound(size_t n) { return 18 * n + LARGE_FIXED; }
 size_t large_arena(size_t n) { return 17 * n + n / 2 + LARGE_FIXED / 2; }
@@ -403,7 +416,10 @@ size_t large_arena(size_t n) { return 17 * n + n / 2 + LARGE_FIXED / 2; }
 // coder stage (at most 12 n + 64 MB) works below it; the inverse ST then takes the whole region in its lean layout (st_decode.cu), and
 // its output lands there too.  26 n + 1 MiB in all, the block included.  The bound adds n / 2 + 255 MiB for what lies outside the
 // arena, as large_bound does: 26.5 n + 256 MiB, 57.2 GB at n = 2146435072.
-size_t large_st_arena(size_t n) { return align_up(n + 128 + 256, 256) + align_up(st_decode_lean_bytes(n), 256); }
+// Below about 5.3 MiB (a routed test block) the block and the coder stage need more than 25 n + 1 MiB: the decoder alone takes 3.4 MB
+// of model state per stream.  The region is then the block plus the coder stage, which stays within the bound.
+size_t large_st_region(size_t n) { return std::max(st_decode_lean_bytes(n), align_up(n + 28 + 128, 256) + need_coder(n)); }
+size_t large_st_arena(size_t n) { return align_up(n + 128 + 256, 256) + align_up(large_st_region(n), 256); }
 size_t large_st_bound(size_t n) { return 26 * n + n / 2 + LARGE_FIXED; }
 
 // run `body(ctx)` on a context of its own, destroyed afterwards so that none of its HBM outlives the call
@@ -591,8 +607,10 @@ int bsc_compress(const unsigned char *input, unsigned char *output, int n, int l
     }
     const bool inplace = (input == output);
     if (n < 0 || n > (inplace ? 2146435072 : 1073741824)) return LIBBSC_BAD_PARAMETER;
-    if (n > LARGE_N) return blockSorter == 1 ? compress_large(output, n, lzpHashSize, lzpMinLen, coder, features) : LIBBSC_NOT_SUPPORTED;
     if (n <= LIBBSC_HEADER_SIZE) return bsc_store(input, output, n, features);
+    // In place only: compress_large works on its argument in place.  Out of place, blocks above 1 GiB were refused above, and below it a
+    // lowered routing threshold (tests) keeps them on the pooled path.
+    if (inplace && n > large_route_n()) return blockSorter == 1 ? compress_large(output, n, lzpHashSize, lzpMinLen, coder, features) : LIBBSC_NOT_SUPPORTED;
     if (lzpMinLen != 0) {                                   // libbsc.cpp:264-276
         unsigned char *lzbuf = (unsigned char *)bsc_malloc((size_t)n + 64);
         if (!lzbuf) return LIBBSC_NOT_ENOUGH_MEMORY;
@@ -632,7 +650,8 @@ int bsc_decompress(const unsigned char *input, int inputSize, unsigned char *out
     if (info != LIBBSC_NO_ERROR) return info;
     if (inputSize < blockSize || outputSize < dataSize) return LIBBSC_UNEXPECTED_EOB;
     unsigned char h[LIBBSC_HEADER_SIZE]; memcpy(h, input, LIBBSC_HEADER_SIZE);
-    if (dataSize > LARGE_N && (get32(h + 8) & 0x1f) >= 3) return decompress_large_st(input, h, blockSize, dataSize, output, features);
+    const bool large = dataSize > large_route_n();
+    if (large && (get32(h + 8) & 0x1f) >= 3) return decompress_large_st(input, h, blockSize, dataSize, output, features);
     // Above 1 GiB (BWT and stored blocks): about 14 n + 64 MB (large_bound holds it), on a context of its own that does not keep it after the call.
     auto body = [&](Ctx *ctx) {
         ctx->arena.reserve((size_t)blockSize + (size_t)dataSize + 8192 + need_coder((size_t)dataSize));      // coder stage, then the inverse BWT in the same space
@@ -646,7 +665,7 @@ int bsc_decompress(const unsigned char *input, int inputSize, unsigned char *out
         if (r == LIBBSC_NO_ERROR && dataSize > 0) { CUDA_TRY(cudaMemcpyAsync(output, d_out, (size_t)dataSize, cudaMemcpyDeviceToHost, ctx->stream)); ctx->sync(); }
         return r;
     };
-    return dataSize > LARGE_N ? with_own_ctx(body) : with_ctx(body);
+    return large ? with_own_ctx(body) : with_ctx(body);
 }
 
 int bsc_bwt_encode(unsigned char *T, int n, unsigned char *num_indexes, int *indexes, int features)

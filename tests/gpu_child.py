@@ -1,5 +1,5 @@
-"""One configuration of tests/test_gpu_pipeline.py, run in a process of its own: the library reads each BSCB200_* switch once per
-process, so every setting needs a fresh one.
+"""One configuration of tests/test_gpu_pipeline.py or tests/test_gpu_large_paths.py, run in a process of its own: the library reads each
+BSCB200_* switch once per process, so every setting needs a fresh one.
 
     python tests/gpu_child.py <job dir>
 
@@ -88,10 +88,24 @@ class Runner:
                 buf = np.zeros(n + 28 + 64, dtype=np.uint8)
                 buf[:n] = a
                 r = self.L.bsc_compress(buf.ctypes.data, buf.ctypes.data, n, lzp[0], lzp[1], args["sorter"], args["coder"], args["features"])
-                out = buf[:r] if r > 0 else None
+                out = buf[:r] if r > 0 else buf                 # on failure the whole buffer: the call must leave it as it was
             else:
                 r, out = b.compress(a, args["sorter"], args["coder"], args["features"], lzp[0], lzp[1])
             self.save(job, r, out)
+        elif op == "raw_decompress":                        # bsc_decompress into n + 64 bytes of 0xA5, all of which come back
+            n = args["n"]
+            buf = np.full(n + 64, 0xA5, dtype=np.uint8)
+            r = self.L.bsc_decompress(a.ctypes.data, a.size, buf.ctypes.data, n, args.get("features", 3))
+            self.save(job, r, buf)
+        elif op == "inplace_decompress":                    # bsc_decompress(buf, size, buf, n) on one buffer, as the reference's CLI calls it
+            n = args["n"]
+            buf = np.zeros(max(n, a.size) + 64, dtype=np.uint8)
+            buf[:a.size] = a
+            r = self.L.bsc_decompress(buf.ctypes.data, a.size, buf.ctypes.data, n, args.get("features", 3))
+            self.save(job, r, buf[:n] if r == 0 else None)
+        elif op == "free_hbm":                              # free HBM once the pooled contexts and sort slabs are released
+            self.L.bscb200_release_pools()
+            self.save(job, 0, free=int(self.L.bscb200_device_free_bytes()))
         elif op == "compress_and_decompress":               # a block too large for a CPU reference: its known answer, then the round trip
             r, blk = b.compress(a, 1, 1, 3)
             self.save(job, r, blk)
