@@ -345,6 +345,28 @@ int block_info_host(const unsigned char *h, int headerSize, int *pBlockSize, int
     return LIBBSC_NO_ERROR;
 }
 
+// The secondary indexes at the end of a BWT block's payload (`payload` bytes at d_payload) for a text of n bytes.  The product's inverse
+// BWT does not use them, but the reference does whenever their count is the one bsc_bwt_encode writes for n (bwt.cpp:295-310), and
+// then libsais_unbwt_aux rejects values outside 0..n - 1 with LIBBSC_BAD_PARAMETER before it decodes.  True for such a block.
+bool secondary_indexes_out_of_range(Ctx *ctx, const u8 *d_payload, int payload, int n, int index)
+{
+    if (n <= 1 || index <= 0 || index > n) return false;                  // stage_bwt_decode answers first, as bsc_bwt_decode does
+    int mod = n / 8;
+    mod |= mod >> 1; mod |= mod >> 2; mod |= mod >> 4; mod |= mod >> 8; mod |= mod >> 16; mod >>= 1;
+    const int want = (unsigned char)((n - 1) / (mod + 1));               // at most 15
+    unsigned char tail[1 + 4 * 16];
+    const int k = payload < (int)sizeof(tail) ? payload : (int)sizeof(tail);
+    CUDA_TRY(cudaMemcpyAsync(tail, d_payload + payload - k, (size_t)k, cudaMemcpyDeviceToHost, ctx->stream));
+    ctx->sync();
+    const int count = tail[k - 1];
+    if (count != want || 4 * count + 1 > k) return false;
+    for (int t = 0; t < count; ++t) {
+        const long long v = (long long)(int)get32(tail + k - 1 - 4 * count + 4 * t) + 1;
+        if (v <= 0 || v > n) return true;
+    }
+    return false;
+}
+
 // bsc_decompress body once the 28-byte header `h` is on the host and the block is in HBM.
 // `lz_out` (host-pointer entry point only): blocks with an LZP stage (mode bits 8..23) are decoded up to the LZP stream, whose
 // length goes to *lz_out; the caller undoes LZP on the host (lzp_host.h) and checks length and Adler-32 of the data there.
@@ -359,11 +381,12 @@ int decompress_dev(Ctx *ctx, const unsigned char *h, const u8 *d_block, int inpu
     const int mode = (int)get32(h + 8);
     if (mode == 0) {
         // A stored block carries exactly dataSize payload bytes (bsc_store, libbsc.cpp:68-81).  The reference copies dataSize bytes
-        // whatever blockSize says (libbsc.cpp:550-555); here a header that promises more data than the block holds is corrupt.
+        // whatever blockSize says (libbsc.cpp:550-555), reading past a shorter block; here such a header is corrupt.  Like the reference,
+        // the data Adler-32 of a stored block is not checked: the payload Adler-32 above covers the same bytes.
         if (payload != dataSize) return LIBBSC_DATA_CORRUPT;
         if (dataSize > 0) CUDA_TRY(cudaMemcpyAsync(d_out, d_block + LIBBSC_HEADER_SIZE, (size_t)dataSize, cudaMemcpyDeviceToDevice, ctx->stream));
         ctx->sync();
-        return get32(h + 16) == get32(h + 20) ? LIBBSC_NO_ERROR : LIBBSC_DATA_CORRUPT;   // same bytes, same checksum
+        return LIBBSC_NO_ERROR;
     }
     const bool lzp = mode != (mode & 0xff);
     if (lzp && !lz_out) return LIBBSC_NOT_SUPPORTED;                     // device-resident API: LZP stays on the host side of the boundary
@@ -373,6 +396,8 @@ int decompress_dev(Ctx *ctx, const unsigned char *h, const u8 *d_block, int inpu
 
     int lzSize = stage_coder_decompress(ctx, d_block + LIBBSC_HEADER_SIZE, payload, d_out, dataSize, coder, features);
     if (lzSize < 0) return lzSize;
+    if (!sorter_valid(sorter)) return LIBBSC_DATA_CORRUPT;               // sorter field 0 with a coder: libbsc.cpp:593, after the coder stage
+    if (sorter == 1 && secondary_indexes_out_of_range(ctx, d_block + LIBBSC_HEADER_SIZE, payload, lzSize, index)) return LIBBSC_BAD_PARAMETER;
     int r;
     if (sorter == 1) r = stage_bwt_decode(ctx, d_out, lzSize, index);
     else { ScratchLease lease(ctx, need_st_decode((size_t)lzSize)); r = stage_st_decode(ctx, d_out, lzSize, sorter, index); }   // libbsc.cpp:584-589
@@ -487,17 +512,20 @@ int compress_large(unsigned char *data, int n, int lzpHashSize, int lzpMinLen, i
 int undo_lzp_host(Ctx *ctx, const unsigned char *h, const u8 *d_lz, int lzSize, unsigned char *output, int dataSize)
 {
     const int mode = (int)get32(h + 8);
-    unsigned char *lz = (unsigned char *)bsc_malloc((size_t)lzSize + 1);
+    // the LZP stream, then the data after it: the caller's buffer is written only once the data is known to be right
+    unsigned char *lz = (unsigned char *)bsc_malloc((size_t)lzSize + (size_t)dataSize + 1);
     if (!lz) return LIBBSC_NOT_ENOUGH_MEMORY;
+    unsigned char *data = lz + lzSize;
     if (lzSize > 0) { CUDA_TRY(cudaMemcpyAsync(lz, d_lz, (size_t)lzSize, cudaMemcpyDeviceToHost, ctx->stream)); ctx->sync(); }
-    int r = lzp_host::decompress(lz, lzSize, output, dataSize, (mode >> 16) & 0xff, (mode >> 8) & 0xff);
+    int r = lzp_host::decompress(lz, lzSize, data, dataSize, (mode >> 16) & 0xff, (mode >> 8) & 0xff);
+    if (r >= 0) r = (r == dataSize && get32(h + 16) == host_adler32(data, (size_t)dataSize)) ? LIBBSC_NO_ERROR : LIBBSC_DATA_CORRUPT;
+    if (r == LIBBSC_NO_ERROR && dataSize > 0) memcpy(output, data, (size_t)dataSize);
     bsc_free(lz);
-    if (r < 0) return r;
-    return (r == dataSize && get32(h + 16) == host_adler32(output, (size_t)dataSize)) ? LIBBSC_NO_ERROR : LIBBSC_DATA_CORRUPT;
+    return r;
 }
 
 // bsc_decompress of a block with block sorter 3..8 whose data size is above 1 GiB (large_st_arena above).  The caller checked the header
-// (block_info_host) and the sizes.  Without LZP the caller's buffer is written only on success.
+// (block_info_host) and the sizes.  The caller's buffer is written only on success.
 int decompress_large_st(const unsigned char *input, const unsigned char *h, int blockSize, int dataSize, unsigned char *output, int features)
 {
     size_t fr = 0, total = 0;
@@ -793,7 +821,7 @@ int bsc_coder_decompress(const unsigned char *input, unsigned char *output, int 
         if (outSize < 0) return LIBBSC_DATA_CORRUPT;
         inSize = (long long)readable_prefix(input, (size_t)outSize + 1 + 16);
     } else {
-        if (nBlocks == 0 || nBlocks > 8) return LIBBSC_DATA_CORRUPT;
+        if (nBlocks > 8) return LIBBSC_DATA_CORRUPT;        // nBlocks == 0: an empty container, 0 bytes (coder.cpp:339-346)
         inSize = 1 + 8 * nBlocks;
         for (int b = 0; b < nBlocks; ++b) { outSize += (int)get32(input + 1 + 8 * b); inSize += (int)get32(input + 5 + 8 * b); }
     }
@@ -961,26 +989,31 @@ int bscb200_bwt_encode_device(void *ctx, unsigned char *d_T, int n, unsigned cha
 int bscb200_bwt_decode_device(void *ctx, unsigned char *d_T, int n, int index)
 {
     Ctx *c = (Ctx *)ctx;
+    if (d_T == nullptr || n < 0 || index <= 0 || index > n) return LIBBSC_BAD_PARAMETER;      // before any workspace is sized from n
     return guarded(c, [&]() { c->arena.reset(); c->arena.reserve(need_bwt_decode((size_t)n)); int r = stage_bwt_decode(c, d_T, n, index); c->sync(); return r; });
 }
 int bscb200_st_encode_device(void *ctx, unsigned char *d_T, int n, int k)
 {
     Ctx *c = (Ctx *)ctx;
+    if (d_T == nullptr || n < 0 || k < 3 || k > 8) return LIBBSC_BAD_PARAMETER;
     return guarded(c, [&]() { c->arena.reset(); ScratchLease lease(c, need_st_encode((size_t)n)); return stage_st_encode(c, d_T, n, k); });
 }
 int bscb200_st_decode_device(void *ctx, unsigned char *d_T, int n, int k, int index)
 {
     Ctx *c = (Ctx *)ctx;
+    if (d_T == nullptr || n < 0 || index < 0 || index >= n || k < 3 || k > 8) return LIBBSC_BAD_PARAMETER;     // st.cpp:1493-1495
     return guarded(c, [&]() { c->arena.reset(); ScratchLease lease(c, need_st_decode((size_t)n)); int r = stage_st_decode(c, d_T, n, k, index); c->sync(); return r; });
 }
 int bscb200_coder_compress_device(void *ctx, const unsigned char *d_in, unsigned char *d_out, int n, int coder, int features)
 {
     Ctx *c = (Ctx *)ctx;
+    if (coder < 1 || coder > 3 || n <= 0) return LIBBSC_BAD_PARAMETER;
     return guarded(c, [&]() { c->arena.reset(); c->arena.reserve(need_coder((size_t)n)); return stage_coder_compress(c, d_in, d_out, n, coder, features); });
 }
 int bscb200_coder_decompress_device(void *ctx, const unsigned char *d_in, int inputSize, unsigned char *d_out, int outputCapacity, int coder, int features)
 {
     Ctx *c = (Ctx *)ctx;
+    if (coder < 1 || coder > 3 || inputSize < 1 || outputCapacity < 0) return LIBBSC_BAD_PARAMETER;
     return guarded(c, [&]() { c->arena.reset(); c->arena.reserve(need_coder((size_t)outputCapacity)); return stage_coder_decompress(c, d_in, inputSize, d_out, outputCapacity, coder, features); });
 }
 unsigned int bscb200_adler32_device(void *ctx, const unsigned char *d_p, int n)

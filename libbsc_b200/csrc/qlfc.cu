@@ -518,12 +518,18 @@ int stage_coder_decompress(Ctx *ctx, const u8 *d_in, int in_size, u8 *d_out, int
         h_sb[0].in_start = 0; h_sb[0].in_size = (u32)out_cap; h_sb[0].out_off = bare ? 0 : 1; h_sb[0].out_cap = (u32)(in_size - (bare ? 0 : 1));
         list[nlist++] = 0;
     } else {
-        if (nBlocks == 0 || nBlocks > Q_MAX_SUB || in_size < 1 + 8 * nBlocks) { A.release(mark); return LIBBSC_DATA_CORRUPT; }
+        if (nBlocks == 0) { A.release(mark); return 0; }   // an empty container decodes to 0 bytes, as in the reference (coder.cpp:339-346)
+        if (nBlocks > Q_MAX_SUB || in_size < 1 + 8 * nBlocks) { A.release(mark); return LIBBSC_DATA_CORRUPT; }
         long long inPtr = 1 + 8 * nBlocks, outPtr = 0;
         for (int b = 0; b < nBlocks; ++b) {
             int rawSize, packed; memcpy(&rawSize, hdr + 1 + 8 * b, 4); memcpy(&packed, hdr + 5 + 8 * b, 4);
-            if (rawSize < 0 || packed < 0 || inPtr + packed > in_size || outPtr + rawSize > out_cap) { A.release(mark); return LIBBSC_DATA_CORRUPT; }
-            h_sb[b].in_start = (u32)outPtr; h_sb[b].in_size = (u32)rawSize; h_sb[b].out_off = (u32)inPtr; h_sb[b].out_cap = (u32)packed;
+            if (rawSize < 0 || packed < 0 || outPtr + rawSize > out_cap) { A.release(mark); return LIBBSC_DATA_CORRUPT; }
+            // Every sub-stream lies inside the payload.  The reference never uses the packed size of the LAST coded sub-block
+            // (coder.cpp:318-336: it only places the sub-blocks after it), so that one is bounded by the payload's end instead of being
+            // rejected; a stored sub-block is copied whole and must fit.
+            const long long avail = in_size - inPtr;
+            if (packed > avail && (b != nBlocks - 1 || packed == rawSize)) { A.release(mark); return LIBBSC_DATA_CORRUPT; }
+            h_sb[b].in_start = (u32)outPtr; h_sb[b].in_size = (u32)rawSize; h_sb[b].out_off = (u32)inPtr; h_sb[b].out_cap = (u32)std::min<long long>(packed, avail);
             if (packed != rawSize) list[nlist++] = (u32)b;
             else { h_sb[b].result = rawSize; if (rawSize) CUDA_TRY(cudaMemcpyAsync(d_out + outPtr, d_in + inPtr, (size_t)rawSize, cudaMemcpyDeviceToDevice, ctx->stream)); }
             inPtr += packed; outPtr += rawSize;

@@ -1,5 +1,5 @@
-"""One configuration of tests/test_gpu_pipeline.py or tests/test_gpu_large_paths.py, run in a process of its own: the library reads each
-BSCB200_* switch once per process, so every setting needs a fresh one.
+"""One configuration of tests/test_gpu_pipeline.py, tests/test_gpu_large_paths.py or tests/test_gpu_malformed.py, run in a process of
+its own: the library reads each BSCB200_* switch once per process, so every setting needs a fresh one.
 
     python tests/gpu_child.py <job dir>
 
@@ -7,6 +7,7 @@ The job dir holds jobs.json (written by the test) and the inputs it names under 
 output to out/<the job's file id>.npy and the return codes, secondary indexes and profile to results.json; the test compares them with the reference.
 Before each job of a serial run it prints "[job] <name>" to stderr, so that the test can tell which [qstats ...] lines belong to which
 job."""
+import hashlib
 import json
 import os
 import random
@@ -103,6 +104,17 @@ class Runner:
             buf[:a.size] = a
             r = self.L.bsc_decompress(buf.ctypes.data, a.size, buf.ctypes.data, n, args.get("features", 3))
             self.save(job, r, buf[:n] if r == 0 else None)
+        elif op == "guarded_decompress":                    # bsc_decompress out of place and in place, with explicit sizes; both buffers whole
+            n, size = args["n"], args["in_size"]
+            buf = np.full(n + 64, 0xA5, dtype=np.uint8)
+            r = self.L.bsc_decompress(a.ctypes.data, size, buf.ctypes.data, n, args.get("features", 3))
+            self.save(job, r, buf)
+            buf = np.full(max(n, a.size) + 64, 0xA5, dtype=np.uint8)
+            buf[:a.size] = a
+            r = self.L.bsc_decompress(buf.ctypes.data, size, buf.ctypes.data, n, args.get("features", 3))
+            self.save(job, r, buf, suffix=".inplace")
+        elif op == "device_guarded":
+            self.device_guarded(job, a, args)
         elif op == "free_hbm":                              # free HBM once the pooled contexts and sort slabs are released
             self.L.bscb200_release_pools()
             self.save(job, 0, free=int(self.L.bscb200_device_free_bytes()))
@@ -141,6 +153,91 @@ class Runner:
             ctx.close()
         else:
             raise ValueError(op)
+
+    GUARD = 4096
+
+    def guarded(self, size, fill):
+        """a device buffer of exactly `size` bytes (filled with `fill`, an array or a byte) at GUARD + off bytes into a tensor whose other
+        bytes hold a known pattern; returns (tensor, start) for offset `off` set by the caller through self._off"""
+        torch = self.torch
+        G, off = self.GUARD, self._off
+        t = (torch.arange(2 * G + off + size, dtype=torch.int32, device="cuda") * 167 + 13).to(torch.uint8)
+        if isinstance(fill, np.ndarray):
+            t[G + off:G + off + size] = torch.from_numpy(np.ascontiguousarray(fill[:size])).cuda()
+        else:
+            t[G + off:G + off + size] = fill
+        return t, G + off
+
+    def guards_intact(self, t, start, size):
+        want = (self.torch.arange(t.numel(), dtype=self.torch.int32, device="cuda") * 167 + 13).to(self.torch.uint8)
+        return bool(self.torch.equal(t[:start], want[:start]) and self.torch.equal(t[start + size:], want[start + size:]))
+
+    def device_guarded(self, job, a, args):
+        """One device-resident entry point on caller buffers of exactly the documented size, at byte offsets 0, 1 and 7 from a 256-byte
+        boundary, each between 4 KiB guards of a known pattern.  Saves the return code and output at offset 0, whether the other offsets
+        gave the same, whether every guard is intact and, for the two decoders, what the host-pointer entry point returns."""
+        torch = self.torch
+        if not hasattr(self, "_ctx"):
+            self._ctx = libbsc_b200.DeviceCtx(0)
+        ctx, call = self._ctx, args["call"]
+        runs = []
+        for off in (0, 1, 7):
+            self._off = off
+            aux = None
+            if call in ("decompress", "coder_decompress"):
+                in_size, cap = args["in_size"], args["out_size"]
+                ti, si = self.guarded(in_size, a)
+                to_, so = self.guarded(cap, 0xA5)
+                torch.cuda.synchronize()
+                if call == "decompress":
+                    r = ctx.decompress(ti.data_ptr() + si, in_size, to_.data_ptr() + so, cap, 3)
+                else:
+                    r = ctx.coder_decompress(ti.data_ptr() + si, in_size, to_.data_ptr() + so, cap, args["coder"], 3)
+                torch.cuda.synchronize()
+                ok = self.guards_intact(ti, si, in_size) and self.guards_intact(to_, so, cap) and torch.equal(ti[si:si + in_size].cpu(), torch.from_numpy(a[:in_size]))
+                out = to_[so:so + cap].cpu().numpy()
+            elif call == "coder_compress":
+                n = a.size
+                ti, si = self.guarded(n, a)
+                to_, so = self.guarded(n + 4096, 0xA5)
+                torch.cuda.synchronize()
+                r = ctx.coder_compress(ti.data_ptr() + si, to_.data_ptr() + so, n, args["coder"], 3)
+                torch.cuda.synchronize()
+                ok = self.guards_intact(ti, si, n) and self.guards_intact(to_, so, n + 4096)
+                out = to_[so:so + max(r, 0)].cpu().numpy()
+            else:                                           # in place on d_T: bwt / st encode / decode, adler32
+                n = a.size
+                t, s = self.guarded(n, a)
+                torch.cuda.synchronize()
+                p = t.data_ptr() + s
+                if call == "bwt_encode":
+                    r, aux = ctx.bwt_encode(p, n)
+                elif call == "bwt_decode":
+                    r = ctx.bwt_decode(p, n, args["index"])
+                elif call == "st_encode":
+                    r = ctx.st_encode(p, n, args["k"])
+                elif call == "st_decode":
+                    r = ctx.st_decode(p, n, args["k"], args["index"])
+                else:
+                    r = ctx.adler32(p, n)
+                torch.cuda.synchronize()
+                ok = self.guards_intact(t, s, n)
+                out = t[s:s + n].cpu().numpy()
+            runs.append((int(r), out, ok, aux))
+        r0, out0, _, aux0 = runs[0]
+        # the output of a failed call is the entry point's working space, not a result: only codes are compared then
+        same = all(r == r0 and x == aux0 and (r0 < 0 or np.array_equal(o, out0)) for r, o, _, x in runs[1:])
+        extra = dict(guards=[ok for _, _, ok, _ in runs], offsets_agree=same, codes=[r for r, _, _, _ in runs], aux=aux0)
+        if call in ("decompress", "coder_decompress"):       # the host entry point's code, and its output where it succeeds
+            buf = np.empty(args["out_size"] + 64, dtype=np.uint8)
+            if call == "decompress":
+                h = int(self.L.bsc_decompress(a.ctypes.data, args["in_size"], buf.ctypes.data, args["out_size"], 3))
+                size = args["out_size"] if h == 0 else -1
+            else:
+                h = int(self.L.bscb200_coder_decompress(a.ctypes.data, args["in_size"], buf.ctypes.data, args["out_size"], args["coder"], 3))
+                size = h
+            extra.update(host=h, host_sha=hashlib.sha256(buf[:size].tobytes()).hexdigest() if size >= 0 else None)
+        self.save(job, r0, out0, **extra)
 
     # ---- modes ----------------------------------------------------------------------------------------------------------------
     def serial(self):
