@@ -128,7 +128,7 @@ int                bscb200_device_count(void);                    /* CUDA device
 long long          bscb200_device_free_bytes(void);               /* free HBM on the current device, -1 on error */
 void               bscb200_release_pools(void);                   /* free the pooled contexts and sort slabs of every device (no call in flight) */
 int                bscb200_set_device(int device);                /* bind the calling thread: all entry points use the current device */
-long long          bscb200_workspace_bytes(int n, int blockSorter);   /* per-context workspace (~13 n + 64 MB): staged block + coder stage */
+long long          bscb200_workspace_bytes(int n, int blockSorter);   /* per-context workspace (~9 n): working copy + coder stage, or the inverse BWT */
 long long          bscb200_workspace_bytes_decode(int n);         /* the same (kept for callers of the round-1 ABI) */
 long long          bscb200_scratch_bytes(int n, int blockSorter);  /* one device-wide sort slab (~58 n for BWT); BSCB200_SORT_SLABS of them per GPU (default 3) */
 /* HBM that an in-place bsc_compress of a block of n > 1 GiB, or bsc_decompress of one, takes at most: 18 n + 256 MiB (about 39 GB at

@@ -207,12 +207,17 @@ template <class F> int guarded(Ctx *c, F body)
     return r;
 }
 
-// arena sizes (bytes) generous enough for each stage at block length n
+// arena sizes (bytes) generous enough for each sort stage at block length n
 size_t need_bwt_encode(size_t n) { return 58 * n + (64u << 20); }
-size_t need_bwt_decode(size_t n) { return 10 * n + (16u << 20); }   // L n, LF 4n, look-back n/2, nodes + 128-byte slabs 3.3 n
 size_t need_st_encode(size_t n)  { return 30 * n + (16u << 20); }
 size_t need_st_decode(size_t n)  { return 41 * n + (16u << 20); }
-size_t need_coder(size_t n)      { return 12 * n + (64u << 20); }
+// The coder stage in either direction, from the buffers it takes (at most about 8.5 n + 28 MB)
+size_t need_coder(size_t n)      { return std::max(coder_compress_bytes((u32)n), coder_decompress_bytes()); }
+// A context's arena on the device-resident entry points: the block's working copy and the coder stage (compress), or the coder stage and
+// then the inverse BWT in the same space (decompress, about 8.7 n).  The sort stages work in the shared slabs.
+size_t ctx_workspace(size_t n)   { return std::max(Arena::bytes_for<u8>(n + 64) + need_coder(n), bwt_decode_bytes((u32)n)); }
+// bsc_compress on a pooled context: the staged block and the output beside that workspace
+size_t host_compress_bytes(size_t n) { return Arena::bytes_for<u8>(n + 64) + Arena::bytes_for<u8>(n + 4096) + ctx_workspace(n); }
 
 unsigned int host_adler32(const unsigned char *p, size_t n)
 {
@@ -413,11 +418,11 @@ int decompress_dev(Ctx *ctx, const unsigned char *h, const u8 *d_block, int inpu
 // On the pooled path a block of n bytes holds about 31 n of HBM: the staged block, its working copy, the output and the coder stage in
 // the context, and a 16.5 n sort slab that the pool keeps after the call.  A block above 1 GiB instead runs on a context made for the
 // call and destroyed after it, in ONE allocation: the block, sorted in place (an in-place call may destroy its input, libbsc.cpp:160),
-// and a region that first holds the batched forward BWT (16 n + 32 B) and then the coder stage with its output (about 13 n + 64 MB).
+// and a region that first holds the batched forward BWT (16 n + 32 B) and then the coder stage with its output (about 9.5 n + 28 MB).
 // The caller's buffer is written only once the block is done.  Only the BWT has a bounded forward sorter: the forward ST needs about
 // 30 n (need_st_encode), so ST3..ST8 compress only up to 1 GiB.  Their inverse has a lean layout (decompress_large_st below).
 // The arena is 17.5 n + 128 MiB: the batched sort at batches of about n / 64 entries (16.5 n) or the coder stage with its output
-// (at most 13 n + 64 MB) after the block.  The bound adds n / 2 + 128 MiB for what lies outside the arena: the context, the coder
+// (at most 9.5 n + 28 MB) after the block.  The bound adds n / 2 + 128 MiB for what lies outside the arena: the context, the coder
 // tables, kernel images loaded on first use and the driver's own transient allocations (about 0.55 GB measured at the largest n).
 constexpr int LARGE_N = 1073741824;                  // blocks above this take the path below
 // Where bsc_compress (in place) and bsc_decompress route: LARGE_N, or BSCB200_LARGE_N=<bytes> (read once per process) when it lies in
@@ -646,7 +651,7 @@ int bsc_compress(const unsigned char *input, unsigned char *output, int n, int l
         if (lzSize >= 0) {
             const LzpInfo lz = {n, host_adler32(input, (size_t)n), (lzpMinLen << 8) | (lzpHashSize << 16)};
             int r = with_ctx([&](Ctx *ctx) {
-                ctx->arena.reserve(3 * (size_t)n + 16384 + need_coder(n));
+                ctx->arena.reserve(host_compress_bytes(n));
                 u8 *d_in = ctx->arena.get<u8>((size_t)lzSize + 64);
                 u8 *d_out = ctx->arena.get<u8>((size_t)n + 4096) + 4;
                 if (lzSize > 0) CUDA_TRY(cudaMemcpyAsync(d_in, lzbuf, (size_t)lzSize, cudaMemcpyHostToDevice, ctx->stream));
@@ -661,7 +666,7 @@ int bsc_compress(const unsigned char *input, unsigned char *output, int n, int l
         bsc_free(lzbuf);                                    // LZP did not shrink the block: continue without it (mode &= 0xff)
     }
     return with_ctx([&](Ctx *ctx) {
-        ctx->arena.reserve(3 * (size_t)n + 16384 + need_coder(n));
+        ctx->arena.reserve(host_compress_bytes(n));
         u8 *d_in = ctx->arena.get<u8>((size_t)n + 64);
         u8 *d_out = ctx->arena.get<u8>((size_t)n + 4096) + 4;      // payload (offset 28) lands 16-byte aligned
         CUDA_TRY(cudaMemcpyAsync(d_in, input, (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
@@ -680,9 +685,10 @@ int bsc_decompress(const unsigned char *input, int inputSize, unsigned char *out
     unsigned char h[LIBBSC_HEADER_SIZE]; memcpy(h, input, LIBBSC_HEADER_SIZE);
     const bool large = dataSize > large_route_n();
     if (large && (get32(h + 8) & 0x1f) >= 3) return decompress_large_st(input, h, blockSize, dataSize, output, features);
-    // Above 1 GiB (BWT and stored blocks): about 14 n + 64 MB (large_bound holds it), on a context of its own that does not keep it after the call.
+    // Above 1 GiB (BWT and stored blocks): about 10.7 n + 28 MB (large_bound holds it), on a context of its own that does not keep it after the call.
     auto body = [&](Ctx *ctx) {
-        ctx->arena.reserve((size_t)blockSize + (size_t)dataSize + 8192 + need_coder((size_t)dataSize));      // coder stage, then the inverse BWT in the same space
+        ctx->arena.reserve(Arena::bytes_for<u8>((size_t)blockSize + 128) + Arena::bytes_for<u8>((size_t)dataSize + 128)
+                           + std::max(need_coder((size_t)dataSize), bwt_decode_bytes((u32)dataSize)));     // coder stage, then the inverse BWT in the same space
         u8 *d_blk = ctx->arena.get<u8>((size_t)blockSize + 128) + 4;
         u8 *d_out = ctx->arena.get<u8>((size_t)dataSize + 128);
         CUDA_TRY(cudaMemcpyAsync(d_blk, input, (size_t)blockSize, cudaMemcpyHostToDevice, ctx->stream));
@@ -716,7 +722,7 @@ int bsc_bwt_decode(unsigned char *T, int n, int index, unsigned char num_indexes
     if (T == nullptr || n < 0 || index <= 0 || index > n) return LIBBSC_BAD_PARAMETER;
     if (n <= 1) return LIBBSC_NO_ERROR;
     return with_ctx([&](Ctx *ctx) {
-        ctx->arena.reserve((size_t)n + 4096 + need_bwt_decode(n));
+        ctx->arena.reserve(Arena::bytes_for<u8>((size_t)n + 64) + bwt_decode_bytes((u32)n));
         u8 *d = ctx->arena.get<u8>((size_t)n + 64);
         CUDA_TRY(cudaMemcpyAsync(d, T, (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
         int r = stage_bwt_decode(ctx, d, n, index);
@@ -899,7 +905,7 @@ int bscb200_ctx_set_sort_budget(void *ctx, long long bytes)
 long long bscb200_workspace_bytes(int n, int blockSorter)
 {
     (void)blockSorter;
-    return (long long)(need_coder((size_t)n) + (size_t)n + 8192);
+    return (long long)ctx_workspace((size_t)n);
 }
 long long bscb200_scratch_bytes(int n, int blockSorter)     /* size of one shared sort slab for blocks of n bytes */
 {
@@ -960,7 +966,7 @@ void bscb200_release_pools(void)
 int bscb200_device_count(void) { int n = 0; return cudaGetDeviceCount(&n) == cudaSuccess ? n : 0; }
 int bscb200_set_device(int device) { return cudaSetDevice(device) == cudaSuccess ? LIBBSC_NO_ERROR : LIBBSC_GPU_ERROR; }
 
-// workspace of a context that only ever DEcompresses blocks of n bytes (inverse BWT + coder stage: ~21 n instead of ~71 n)
+// workspace of a context that only ever DEcompresses blocks of n bytes: the same as bscb200_workspace_bytes
 long long bscb200_workspace_bytes_decode(int n) { return bscb200_workspace_bytes(n, 1); }
 unsigned long long bscb200_ctx_kernel_launches(void *ctx) { return ((Ctx *)ctx)->kernels_launched; }
 
@@ -990,7 +996,7 @@ int bscb200_bwt_decode_device(void *ctx, unsigned char *d_T, int n, int index)
 {
     Ctx *c = (Ctx *)ctx;
     if (d_T == nullptr || n < 0 || index <= 0 || index > n) return LIBBSC_BAD_PARAMETER;      // before any workspace is sized from n
-    return guarded(c, [&]() { c->arena.reset(); c->arena.reserve(need_bwt_decode((size_t)n)); int r = stage_bwt_decode(c, d_T, n, index); c->sync(); return r; });
+    return guarded(c, [&]() { c->arena.reset(); c->arena.reserve(bwt_decode_bytes((u32)n)); int r = stage_bwt_decode(c, d_T, n, index); c->sync(); return r; });
 }
 int bscb200_st_encode_device(void *ctx, unsigned char *d_T, int n, int k)
 {

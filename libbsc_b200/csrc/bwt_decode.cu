@@ -87,7 +87,19 @@ __global__ void __launch_bounds__(256) unbwt_place(const u64 *__restrict__ pair,
     }
 }
 
+// one segment per window of 64 rows (mark_row); every further node of a segment holds 64 bytes of text
+u32 unbwt_segments(u32 n) { return ceil_div((u64)n + 1, 64); }
+u32 unbwt_max_nodes(u32 n) { return unbwt_segments(n) + n / UW_SLAB + 2; }
+
 }  // namespace
+
+size_t bwt_decode_bytes(u32 n)
+{
+    const size_t nodes = unbwt_max_nodes(n);
+    return Arena::bytes_for<u8>((size_t)n + 64) + Arena::bytes_for<u32>((size_t)n + 2) + Arena::bytes_for<u32>(256 + 64 + 64)
+         + Arena::bytes_for<u64>((size_t)ceil_div(n, LF_TILE) * 256) + Arena::bytes_for<u64>(nodes) + Arena::bytes_for<u8>(nodes)
+         + Arena::bytes_for<u32>(nodes * (UW_SLAB / 4));
+}
 
 int stage_bwt_decode(Ctx *ctx, u8 *d_T, int n_, int index_)
 {
@@ -97,9 +109,10 @@ int stage_bwt_decode(Ctx *ctx, u8 *d_T, int n_, int index_)
     Arena &A = ctx->arena;
     const size_t mark = A.mark();
 
+    // the buffers below are what bwt_decode_bytes(n) counts
     const u32 tiles = ceil_div(n, LF_TILE);
-    const u32 K = ceil_div((u64)n + 1, 64);                  // one segment per window of 64 rows (mark_row)
-    const u32 max_nodes = K + n / UW_SLAB + 2;               // every further node of a segment holds 64 bytes of text
+    const u32 K = unbwt_segments(n);
+    const u32 max_nodes = unbwt_max_nodes(n);
     u8  *Lp    = A.get<u8>((size_t)n + 64);
     u32 *LF    = A.get<u32>((size_t)n + 2);
     u32 *hist  = A.get<u32>(256 + 64 + 64);                  // [0..255] counts / bases, [256] tile counter, [320] node counter, [321..] jump flags

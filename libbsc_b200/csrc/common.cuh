@@ -79,8 +79,10 @@ struct Arena {
         if (e != cudaSuccess) { cudaGetLastError(); throw CudaFail{cudaErrorMemoryAllocation, __FILE__, __LINE__}; }
         cap = bytes;
     }
+    // what get<T>(count) takes from the arena: 256 B slack after every buffer, 256-byte aligned
+    template <typename T> static size_t bytes_for(size_t count) { return align_up(count * sizeof(T) + 256, 256); }
     template <typename T> T *get(size_t count) {
-        size_t bytes = align_up(count * sizeof(T) + 256, 256);      // 256 B slack after every buffer
+        size_t bytes = bytes_for<T>(count);
         if (used + bytes > cap) throw CudaFail{cudaErrorMemoryAllocation, __FILE__, __LINE__};
         T *p = (T *)(base + used); used += bytes; return p;
     }

@@ -217,6 +217,24 @@ static int coder_num_blocks(int n)                        // coder.cpp:52-59
     return 8;
 }
 
+// The most stage_coder_compress takes from ctx->arena for n input bytes (a bare output capacity of at most n), whatever the data: every
+// byte a run (R = n), the rank tables of that many runs, the models of the most sub-blocks and the clipped re-encodes of the serial rules.
+size_t coder_compress_bytes(u32 n)
+{
+    const size_t R = n, rank_tiles = ceil_div(R, RK_TILE) + Q_MAX_SUB;        // every sub-block rounds its tiles up
+    return Arena::bytes_for<u32>(2 * Q_MAX_SUB) + Arena::bytes_for<SubBlock>(Q_MAX_SUB) + Arena::bytes_for<u32>(ceil_div(n, RUN_TILE) + 1)
+         + Arena::bytes_for<u8>(256 * Q_MAX_SUB) + Arena::bytes_for<short>(Q_MAX_SUB * MODEL_SHORTS_PAD)
+         + Arena::bytes_for<u8>((size_t)n + (4096 + 256) * Q_MAX_SUB)
+         + Arena::bytes_for<u32>(R + 2) + 2 * Arena::bytes_for<u8>(R + 32) + Arena::bytes_for<u32>(Q_MAX_SUB)
+         + 2 * Arena::bytes_for<u32>(rank_tiles * 256) + Q_MAX_SUB * Arena::bytes_for<u32>(1);
+}
+
+// The most stage_coder_decompress takes from ctx->arena: the sub-block table and the models of the most streams a container can hold.
+size_t coder_decompress_bytes()
+{
+    return Arena::bytes_for<SubBlock>(Q_MAX_SUB) + Arena::bytes_for<u32>(Q_MAX_SUB) + Arena::bytes_for<short>(Q_MAX_SUB * MODEL_SHORTS_PAD);
+}
+
 // ONE copy of the constant tables per device (never freed: 58 KB), shared by every context: the coders that read the state tables
 // through L1 (LayoutDietTG) then share their cache lines between the CTAs of different blocks on an SM.
 static const QTables *get_tables(Ctx *ctx)

@@ -14,8 +14,9 @@ size_t bwt_batched_bytes(u32 n, u32 B);
 u32 bwt_batch_floor(u32 n);
 // batch entries that a working set of `budget` bytes allows at block length n (at least bwt_batch_floor(n), at most that or n)
 u32 bwt_batch_entries(u32 n, long long budget);
-// Inverse BWT in place (bsc_bwt_decode, bwt.cpp:283).
+// Inverse BWT in place (bsc_bwt_decode, bwt.cpp:283).  Takes bwt_decode_bytes(n) from ctx->arena.
 int stage_bwt_decode(Ctx *ctx, u8 *d_T, int n, int index);
+size_t bwt_decode_bytes(u32 n);
 // Sort transform of order k in place (bsc_st_encode, st.cpp:990; k = 3..8).
 int stage_st_encode(Ctx *ctx, u8 *d_T, int n, int k);
 // Inverse sort transform in place (bsc_st_decode, st.cpp:1491; k = 3..8, index = row of rotation 0).
@@ -31,6 +32,9 @@ int stage_coder_compress(Ctx *ctx, const u8 *d_in, u8 *d_out, int n, int coder, 
 // bsc_coder_decompress (coder.cpp:273).  `in_size` bounds the readable input (device padded by >= 64 bytes);
 // out_cap bounds the writable output.
 int stage_coder_decompress(Ctx *ctx, const u8 *d_in, int in_size, u8 *d_out, int out_cap, int coder, int features, bool bare = false);   // bare: one stream, no container byte
+// the most each coder stage takes from ctx->arena, over every input (qlfc.cu)
+size_t coder_compress_bytes(u32 n);
+size_t coder_decompress_bytes();
 // Adler-32 of a device buffer (bsc_adler32, adler32.cpp:83).  Result lands in ctx->d_mail[slot]
 // (asynchronously); adler32_fetch() waits and returns it.
 void stage_adler32_async(Ctx *ctx, const u8 *d_p, int n, int slot);
