@@ -29,8 +29,6 @@ namespace {
 constexpr int MAX_DEVICES = 16;
 std::mutex g_pool_mutex;
 std::vector<Ctx *> g_pool[MAX_DEVICES];
-bool g_initialised = false;
-int g_features = 0;
 void *(*g_malloc)(size_t) = nullptr;
 void *(*g_zero_malloc)(size_t) = nullptr;
 void (*g_free)(void *) = nullptr;
@@ -55,14 +53,15 @@ Ctx *ctx_new(int device, cudaStream_t stream, bool own)
     return c;
 }
 
+// Destroys a context; its kernel launches stay counted in bscb200_total_kernel_launches.
 void ctx_delete(Ctx *c)
 {
     if (!c) return;
+    { std::lock_guard<std::mutex> lk(g_pool_mutex); g_launches_retired += c->kernels_launched; }
     cudaSetDevice(c->device);
     c->arena.destroy();
     if (c->h_mail) cudaFreeHost(c->h_mail);
     if (c->d_mail) cudaFree(c->d_mail);
-    if (c->h_stage) cudaFreeHost(c->h_stage);
     for (cudaEvent_t e : c->ev_pool) cudaEventDestroy(e);
     if (c->stream_hi) cudaStreamDestroy(c->stream_hi);
     if (c->stream_lo) cudaStreamDestroy(c->stream_lo);
@@ -108,6 +107,16 @@ int scratch_limit()
     return v;
 }
 
+// Frees a slab (null: nothing) once its last user is done with it.
+void scratch_destroy(Scratch *s)
+{
+    if (!s) return;
+    if (s->idle_valid) cudaEventSynchronize(s->idle);
+    s->arena.destroy();
+    if (s->idle) cudaEventDestroy(s->idle);
+    delete s;
+}
+
 Scratch *scratch_acquire(Ctx *c, size_t bytes)
 {
     ScratchPool &P = g_scratch[c->device];
@@ -133,12 +142,12 @@ Scratch *scratch_acquire(Ctx *c, size_t bytes)
             std::unique_lock<std::mutex> lk(P.m);
             if (fresh && f.err == cudaErrorMemoryAllocation && P.created > 1) {       // no room for one more slab: live with the ones there are
                 cudaGetLastError();
-                if (s) { if (s->idle) cudaEventDestroy(s->idle); s->arena.destroy(); delete s; }
+                scratch_destroy(s);
                 P.created--; P.cap = P.created;
                 P.cv.notify_all();
                 continue;
             }
-            if (s && !fresh) { P.free_list.push_back(s); } else { if (s) { if (s->idle) cudaEventDestroy(s->idle); s->arena.destroy(); delete s; } P.created--; }
+            if (fresh) { scratch_destroy(s); P.created--; } else P.free_list.push_back(s);
             P.cv.notify_one();
             throw;
         } catch (...) {
@@ -170,40 +179,54 @@ struct ScratchLease {
     ScratchLease(const ScratchLease &) = delete; ScratchLease &operator=(const ScratchLease &) = delete;
 };
 
-int map_failure(const CudaFail &f)
+// ---- the three context lifetimes of an entry point ------------------------------------------------------------------------------
+// Runs `body()` and returns its result, or the libbsc code of what it threw: nothing may unwind through the extern "C" boundary.
+// `failed` tells whether it threw, which may leave the context mid-stage.
+template <class F> int run_mapped(F &&body, bool &failed)
 {
-    cudaGetLastError();
-    return f.err == cudaErrorMemoryAllocation ? LIBBSC_GPU_NOT_ENOUGH_MEMORY : LIBBSC_GPU_ERROR;
+    failed = true;
+    int r;
+    try { r = body(); failed = false; }
+    catch (const CudaFail &f) { cudaGetLastError(); r = f.err == cudaErrorMemoryAllocation ? LIBBSC_GPU_NOT_ENOUGH_MEMORY : LIBBSC_GPU_ERROR; }
+    catch (const std::bad_alloc &) { r = LIBBSC_NOT_ENOUGH_MEMORY; }
+    catch (...) { r = LIBBSC_GPU_ERROR; }
+    return r;
 }
 
-// run `body(ctx)` on a pooled context, translating CUDA failures into libbsc error codes.  Nothing may unwind through the
-// extern "C" boundary, and a context that failed mid-stage is destroyed instead of pooled (its device mailbox may hold partial
-// Adler-32 sums that the next block would inherit).
+// run `body(ctx)` on a pooled context.  A context that failed mid-stage is destroyed instead of pooled (its device mailbox may hold
+// partial Adler-32 sums that the next block would inherit).
 template <class F> int with_ctx(F body)
 {
     Ctx *c = ctx_acquire();
     if (!c) return LIBBSC_GPU_NOT_SUPPORTED;
-    int r; bool broken = true;
-    try { r = body(c); broken = false; }
-    catch (const CudaFail &f) { r = map_failure(f); }
-    catch (const std::bad_alloc &) { r = LIBBSC_NOT_ENOUGH_MEMORY; }
-    catch (...) { r = LIBBSC_GPU_ERROR; }
-    if (broken) {
-        cudaStreamSynchronize(c->stream); cudaGetLastError();
-        { std::lock_guard<std::mutex> lk(g_pool_mutex); g_launches_retired += c->kernels_launched; }
-        ctx_delete(c);
-    } else ctx_release(c);
+    bool failed;
+    const int r = run_mapped([&] { return body(c); }, failed);
+    if (failed) { cudaStreamSynchronize(c->stream); cudaGetLastError(); ctx_delete(c); }
+    else ctx_release(c);
     return r;
 }
+
+// run `body(ctx)` on a context of its own, destroyed afterwards so that none of its HBM outlives the call
+template <class F> int with_own_ctx(F body)
+{
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess) { cudaGetLastError(); return LIBBSC_GPU_NOT_SUPPORTED; }
+    Ctx *c = nullptr;
+    bool failed;
+    const int r = run_mapped([&] { c = ctx_new(dev, nullptr, true); return body(c); }, failed);
+    if (c) { cudaStreamSynchronize(c->stream); cudaGetLastError(); ctx_delete(c); }
+    return r;
+}
+
+// run `body()` on the caller's context, which a failure leaves reset for its next call
 template <class F> int guarded(Ctx *c, F body)
 {
-    int r;
-    try { return body(); }
-    catch (const CudaFail &f) { r = map_failure(f); }
-    catch (const std::bad_alloc &) { r = LIBBSC_NOT_ENOUGH_MEMORY; }
-    catch (...) { r = LIBBSC_GPU_ERROR; }
-    cudaStreamSynchronize(c->stream); cudaGetLastError(); c->arena.reset();
-    cudaMemsetAsync(c->d_mail, 0, 1024, c->stream); cudaStreamSynchronize(c->stream); cudaGetLastError();   // adler32.cu expects zeroed accumulators
+    bool failed;
+    const int r = run_mapped(body, failed);
+    if (failed) {
+        cudaStreamSynchronize(c->stream); cudaGetLastError(); c->arena.reset();
+        cudaMemsetAsync(c->d_mail, 0, 1024, c->stream); cudaStreamSynchronize(c->stream); cudaGetLastError();   // adler32.cu expects zeroed accumulators
+    }
     return r;
 }
 
@@ -218,6 +241,12 @@ size_t need_coder(size_t n)      { return std::max(coder_compress_bytes((u32)n),
 size_t ctx_workspace(size_t n)   { return std::max(Arena::bytes_for<u8>(n + 64) + need_coder(n), bwt_decode_bytes((u32)n)); }
 // bsc_compress on a pooled context: the staged block and the output beside that workspace
 size_t host_compress_bytes(size_t n) { return Arena::bytes_for<u8>(n + 64) + Arena::bytes_for<u8>(n + 4096) + ctx_workspace(n); }
+// bsc_decompress of a block of `block` bytes that holds n bytes of data: the staged block and the output beside the coder stage, then
+// the inverse BWT in the same space.  Above 1 GiB (BWT and stored blocks) this is about 10.7 n + 28 MB, which large_bound holds.
+size_t host_decompress_bytes(size_t block, size_t n)
+{
+    return Arena::bytes_for<u8>(block + 128) + Arena::bytes_for<u8>(n + 128) + std::max(need_coder(n), bwt_decode_bytes((u32)n));
+}
 
 unsigned int host_adler32(const unsigned char *p, size_t n)
 {
@@ -241,7 +270,53 @@ size_t readable_prefix(const void *p, size_t want)
     return ok < want ? ok : want;
 }
 
+// the parameter ranges of libbsc: arguments outside them are LIBBSC_BAD_PARAMETER, header fields outside them LIBBSC_DATA_CORRUPT
 bool sorter_valid(int s) { return s == 1 || (s >= 3 && s <= 8); }
+bool coder_valid(int c) { return c >= 1 && c <= 3; }
+bool lzp_valid(int hash, int min) { return hash >= 10 && hash <= 28 && min >= 4 && min <= 255; }
+bool st_order_valid(int k) { return k >= 3 && k <= 8; }
+
+// ---- the 28-byte block header (libbsc.cpp:68-81, 340-418) ------------------------------------------------------------------------
+// The mode word: block sorter in bits 0..4, coder in 5..7, LZP minimum length in 8..15, LZP hash size in 16..23; 0 for a stored block.
+struct Mode {
+    int word = 0;
+    static Mode of(int sorter, int coder, int lzpHash, int lzpMin) { return Mode{sorter | (coder << 5) | (lzpMin << 8) | (lzpHash << 16)}; }
+    int sorter() const { return word & 0x1f; }
+    int coder() const { return (word >> 5) & 7; }
+    int lzp_min() const { return (word >> 8) & 0xff; }
+    int lzp_hash() const { return (word >> 16) & 0xff; }
+    bool has_lzp() const { return word != (word & 0xff); }
+};
+
+struct BlockHeader {
+    int block_size = 0, data_size = 0;
+    Mode mode;
+    int index = 0;
+    u32 adler_data = 0, adler_payload = 0;
+
+    int payload() const { return block_size - LIBBSC_HEADER_SIZE; }
+    // the 28 bytes at h, the header's own Adler-32 last
+    void write(unsigned char *h) const
+    {
+        put32(h, (u32)block_size); put32(h + 4, (u32)data_size); put32(h + 8, (u32)mode.word); put32(h + 12, (u32)index);
+        put32(h + 16, adler_data); put32(h + 20, adler_payload); put32(h + 24, host_adler32(h, 24));
+    }
+    // Reads the header at h (headerSize readable bytes) with bsc_block_info's checks, its codes in its order.
+    int read(const unsigned char *h, int headerSize)
+    {
+        if (headerSize < LIBBSC_HEADER_SIZE) return LIBBSC_UNEXPECTED_EOB;
+        if (get32(h + 24) != host_adler32(h, 24)) return LIBBSC_DATA_CORRUPT;
+        *this = BlockHeader{(int)get32(h), (int)get32(h + 4), Mode{(int)get32(h + 8)}, (int)get32(h + 12), get32(h + 16), get32(h + 20)};
+        const Mode m = mode;
+        if (m.sorter() != 0 && !sorter_valid(m.sorter())) return LIBBSC_DATA_CORRUPT;
+        if (m.coder() != 0 && !coder_valid(m.coder())) return LIBBSC_DATA_CORRUPT;
+        if ((m.lzp_min() != 0 || m.lzp_hash() != 0) && !lzp_valid(m.lzp_hash(), m.lzp_min())) return LIBBSC_DATA_CORRUPT;
+        if (Mode::of(m.sorter(), m.coder(), m.lzp_hash(), m.lzp_min()).word != m.word) return LIBBSC_DATA_CORRUPT;    // bits 24..31 set
+        if (block_size < LIBBSC_HEADER_SIZE || block_size > LIBBSC_HEADER_SIZE + data_size) return LIBBSC_DATA_CORRUPT;
+        if (index < 0 || index > data_size) return LIBBSC_DATA_CORRUPT;
+        return LIBBSC_NO_ERROR;
+    }
+};
 
 // Forward BWT of a block on this context, its sort in a shared slab: the standard sorter, or the batched one when the context's sort
 // budget (bscb200_ctx_set_sort_budget) is smaller than the standard working set.
@@ -257,96 +332,129 @@ int bwt_encode_leased(Ctx *ctx, u8 *d_T, int n, unsigned char *num_indexes, int 
 }
 
 // ---------------------------------------------------------------------------------------------
-// device-resident block compress / decompress
+// block compress
 // ---------------------------------------------------------------------------------------------
 // Stored block (libbsc.cpp:68-81) built on the device: header on host, data D2D.
 int store_dev(Ctx *ctx, const u8 *d_in, int n, u8 *d_out, u32 adler_data)
 {
-    unsigned char h[LIBBSC_HEADER_SIZE];
-    put32(h, (u32)(n + LIBBSC_HEADER_SIZE)); put32(h + 4, (u32)n); put32(h + 8, 0); put32(h + 12, 0);
-    put32(h + 16, adler_data); put32(h + 20, adler_data); put32(h + 24, host_adler32(h, 24));
     if (n > 0) CUDA_TRY(cudaMemcpyAsync(d_out + LIBBSC_HEADER_SIZE, d_in, (size_t)n, cudaMemcpyDeviceToDevice, ctx->stream));
-    memcpy(ctx->h_mail + 64, h, LIBBSC_HEADER_SIZE);
+    BlockHeader{n + LIBBSC_HEADER_SIZE, n, Mode{0}, 0, adler_data, adler_data}.write((unsigned char *)(ctx->h_mail + 64));
     CUDA_TRY(cudaMemcpyAsync(d_out, ctx->h_mail + 64, LIBBSC_HEADER_SIZE, cudaMemcpyHostToDevice, ctx->stream));
     ctx->sync();
     return n + LIBBSC_HEADER_SIZE;
 }
 
-// bsc_compress with LZP disabled, everything in HBM.  d_out must hold n + 28 bytes.
-// `lz` (host-pointer bsc_compress with LZP parameters only): d_in holds the LZP stream of a block of lz->orig_n bytes whose Adler-32
-// is lz->adler_orig; the header describes the original block, and a block that does not shrink is reported as LIBBSC_NOT_COMPRESSIBLE
-// (the caller stores the ORIGINAL data, libbsc.cpp:315-318).
-struct LzpInfo { int orig_n; u32 adler_orig; int mode_bits; };
-int finish_dev(Ctx *ctx, u8 *d_out, int result, unsigned char num_indexes, const int *indexes, int orig_n, int mode, int index, u32 adler_data);
+// The LZP stage of a block before compression, on the host and not in place (libbsc.cpp:139-154, 264-276).  After run(), `stream` holds
+// the LZP stream of the block, or is null: LZP was not asked for, or it did not shrink the block, which goes on without it (mode &= 0xff).
+struct LzpPass {
+    unsigned char *stream = nullptr;
+    int size = 0, hash = 0, min = 0, orig_n = 0;
+    u32 adler_orig = 0;
 
-int compress_dev(Ctx *ctx, const u8 *d_in, int n, u8 *d_out, int blockSorter, int coder, int features, bool inplace_rules, const LzpInfo *lz = nullptr)
+    LzpPass() = default;
+    LzpPass(const LzpPass &) = delete; LzpPass &operator=(const LzpPass &) = delete;
+    ~LzpPass() { if (stream) bsc_free(stream); }
+    int run(const unsigned char *data, int n, int lzpHashSize, int lzpMinLen, int features)
+    {
+        if (lzpMinLen == 0) return LIBBSC_NO_ERROR;
+        stream = (unsigned char *)bsc_malloc((size_t)n + 64);
+        if (!stream) return LIBBSC_NOT_ENOUGH_MEMORY;
+        size = lzp_host::compress(data, stream, n, lzpHashSize, lzpMinLen, (features & LIBBSC_FEATURE_MULTITHREADING) != 0);
+        if (size < 0) { bsc_free(stream); stream = nullptr; return LIBBSC_NO_ERROR; }
+        hash = lzpHashSize; min = lzpMinLen; orig_n = n; adler_orig = host_adler32(data, (size_t)n);
+        return LIBBSC_NO_ERROR;
+    }
+};
+
+// The rest of a block once the coder stage returned `result` (its output at d_out + 28, or a code), as libbsc.cpp:181-210 and 311-337
+// frame it: LIBBSC_NOT_COMPRESSIBLE unless the block shrinks, else the secondary indexes after the coder output and the header.  H
+// describes the block but for its size and the payload Adler-32.  Returns the block's size.
+int finish_dev(Ctx *ctx, u8 *d_out, int result, unsigned char num_indexes, const int *indexes, BlockHeader H)
 {
-    if (!sorter_valid(blockSorter)) return LIBBSC_BAD_PARAMETER;
-    if (coder < 1 || coder > 3) return LIBBSC_BAD_PARAMETER;
+    if (result == LIBBSC_NOT_SUPPORTED) return result;
+    if (result < 0 || result + 1 + 4 * num_indexes >= H.data_size) return LIBBSC_NOT_COMPRESSIBLE;
+    unsigned char *tail = (unsigned char *)(ctx->h_mail + 96);            // pinned, <= 4*255+1 bytes needs care: num_indexes <= 15 here
+    memcpy(tail, indexes, 4 * (size_t)num_indexes);
+    tail[4 * num_indexes] = num_indexes;
+    CUDA_TRY(cudaMemcpyAsync(d_out + LIBBSC_HEADER_SIZE + result, tail, 4 * (size_t)num_indexes + 1, cudaMemcpyHostToDevice, ctx->stream));
+    result += 1 + 4 * num_indexes;
+    H.block_size = result + LIBBSC_HEADER_SIZE;
+    H.adler_payload = stage_adler32(ctx, d_out + LIBBSC_HEADER_SIZE, result);
+    unsigned char *h = (unsigned char *)(ctx->h_mail + 64);
+    H.write(h);
+    CUDA_TRY(cudaMemcpyAsync(d_out, h, LIBBSC_HEADER_SIZE, cudaMemcpyHostToDevice, ctx->stream));
+    ctx->sync();
+    return H.block_size;
+}
+
+// bsc_compress with LZP disabled, everything in HBM.  d_out must hold n + 28 bytes.
+// `lz` (host-pointer bsc_compress with LZP parameters only): d_in holds the LZP stream of a block of lz->orig_n bytes; the header describes
+// the original block, and a block that does not shrink is reported as LIBBSC_NOT_COMPRESSIBLE (the caller stores the ORIGINAL data,
+// libbsc.cpp:315-318).
+int compress_dev(Ctx *ctx, const u8 *d_in, int n, u8 *d_out, int blockSorter, int coder, int features, bool inplace_rules, const LzpPass *lz = nullptr)
+{
+    if (!sorter_valid(blockSorter) || !coder_valid(coder)) return LIBBSC_BAD_PARAMETER;
     if (n < 0 || n > 1073741824) return LIBBSC_BAD_PARAMETER;
     if (lz && n <= LIBBSC_HEADER_SIZE) blockSorter = 1;                  // libbsc.cpp:278-282: a tiny LZP stream is always BWT-sorted
-    int mode = blockSorter | (coder << 5) | (lz ? lz->mode_bits : 0);
-    const u32 adler_data = lz ? lz->adler_orig : stage_adler32(ctx, d_in, n);
-    if (!lz && n <= LIBBSC_HEADER_SIZE) return store_dev(ctx, d_in, n, d_out, adler_data);
-    const int orig_n = lz ? lz->orig_n : n;
+    BlockHeader H;
+    H.data_size = lz ? lz->orig_n : n;
+    H.mode = Mode::of(blockSorter, coder, lz ? lz->hash : 0, lz ? lz->min : 0);
+    H.adler_data = lz ? lz->adler_orig : stage_adler32(ctx, d_in, n);
+    if (!lz && n <= LIBBSC_HEADER_SIZE) return store_dev(ctx, d_in, n, d_out, H.adler_data);
 
     Arena &A = ctx->arena;
     const size_t mark = A.mark();
     u8 *work = A.get<u8>((size_t)n + 64);
     CUDA_TRY(cudaMemcpyAsync(work, d_in, (size_t)n, cudaMemcpyDeviceToDevice, ctx->stream));
 
-    int indexes[256]; unsigned char num_indexes = 0; int index;
-    if (blockSorter == 1) index = bwt_encode_leased(ctx, work, n, &num_indexes, indexes);      // the sort's ~58 n live in a shared slab
-    else { ScratchLease lease(ctx, need_st_encode(n)); index = stage_st_encode(ctx, work, n, blockSorter); }
-    if (orig_n < 64 * 1024) num_indexes = 0;              // libbsc.cpp:303
-    if (index < 0) { A.release(mark); return index; }
+    int indexes[256]; unsigned char num_indexes = 0;
+    if (blockSorter == 1) H.index = bwt_encode_leased(ctx, work, n, &num_indexes, indexes);      // the sort's ~58 n live in a shared slab
+    else { ScratchLease lease(ctx, need_st_encode(n)); H.index = stage_st_encode(ctx, work, n, blockSorter); }
+    if (H.data_size < 64 * 1024) num_indexes = 0;       // libbsc.cpp:303
+    if (H.index < 0) { A.release(mark); return H.index; }
 
-    int result = stage_coder_compress(ctx, work, d_out + LIBBSC_HEADER_SIZE, n, coder, features);
+    const int result = stage_coder_compress(ctx, work, d_out + LIBBSC_HEADER_SIZE, n, coder, features);
     A.release(mark);
-    if (result == LIBBSC_NOT_SUPPORTED) return result;
-    if (result < 0 || result + 1 + 4 * num_indexes >= orig_n) {
-        if (inplace_rules || lz) return LIBBSC_NOT_COMPRESSIBLE;         // libbsc.cpp:188-191
-        return store_dev(ctx, d_in, n, d_out, adler_data);               // libbsc.cpp:315-318
-    }
-    return finish_dev(ctx, d_out, result, num_indexes, indexes, orig_n, mode, index, adler_data);
+    const int size = finish_dev(ctx, d_out, result, num_indexes, indexes, H);
+    if (size == LIBBSC_NOT_COMPRESSIBLE && !inplace_rules && !lz) return store_dev(ctx, d_in, n, d_out, H.adler_data);   // libbsc.cpp:315-318
+    return size;
 }
 
-// The secondary indexes and the header of a compressed block whose coder output (`result` bytes) is at d_out + 28.
-int finish_dev(Ctx *ctx, u8 *d_out, int result, unsigned char num_indexes, const int *indexes, int orig_n, int mode, int index, u32 adler_data)
+// ---------------------------------------------------------------------------------------------
+// block decompress, step by step (libbsc.cpp:522-617).  The callers checked the header H (BlockHeader::read) and the sizes, and the
+// block's payload lies at d_payload with 64 readable bytes after it.  Only the inverse sort and where the buffers sit differ by path.
+// ---------------------------------------------------------------------------------------------
+// The coder stage into d_L: returns the length of the sorted (and LZP-coded) data or a code.  A stored block may be empty, so the
+// empty payload is rejected here, after the stored blocks have left.
+int decode_coder(Ctx *ctx, const BlockHeader &H, const u8 *d_payload, u8 *d_L, int features)
 {
-    unsigned char *tail = (unsigned char *)(ctx->h_mail + 96);            // pinned, <= 4*255+1 bytes needs care: num_indexes <= 15 here
-    memcpy(tail, indexes, 4 * (size_t)num_indexes);
-    tail[4 * num_indexes] = num_indexes;
-    CUDA_TRY(cudaMemcpyAsync(d_out + LIBBSC_HEADER_SIZE + result, tail, 4 * (size_t)num_indexes + 1, cudaMemcpyHostToDevice, ctx->stream));
-    result += 1 + 4 * num_indexes;
-    const u32 adler_payload = stage_adler32(ctx, d_out + LIBBSC_HEADER_SIZE, result);
-    unsigned char *h = (unsigned char *)(ctx->h_mail + 64);
-    put32(h, (u32)(result + LIBBSC_HEADER_SIZE)); put32(h + 4, (u32)orig_n); put32(h + 8, (u32)mode); put32(h + 12, (u32)index);
-    put32(h + 16, adler_data); put32(h + 20, adler_payload); put32(h + 24, host_adler32(h, 24));
-    CUDA_TRY(cudaMemcpyAsync(d_out, h, LIBBSC_HEADER_SIZE, cudaMemcpyHostToDevice, ctx->stream));
-    ctx->sync();
-    return result + LIBBSC_HEADER_SIZE;
+    if (H.payload() < 1) return LIBBSC_DATA_CORRUPT;
+    return stage_coder_decompress(ctx, d_payload, H.payload(), d_L, H.data_size, H.mode.coder(), features);
 }
 
-int block_info_host(const unsigned char *h, int headerSize, int *pBlockSize, int *pDataSize)
+// libbsc.cpp:599-613: undo the LZP stage of a block on the host, from the lzSize-byte LZP stream at d_lz
+int undo_lzp_host(Ctx *ctx, const BlockHeader &H, const u8 *d_lz, int lzSize, unsigned char *output)
 {
-    if (headerSize < LIBBSC_HEADER_SIZE) return LIBBSC_UNEXPECTED_EOB;
-    if (get32(h + 24) != host_adler32(h, 24)) return LIBBSC_DATA_CORRUPT;
-    int blockSize = (int)get32(h), dataSize = (int)get32(h + 4), mode = (int)get32(h + 8), index = (int)get32(h + 12);
-    int lzpHash = (mode >> 16) & 0xff, lzpMin = (mode >> 8) & 0xff, coder = (mode >> 5) & 7, sorter = mode & 0x1f;
-    int rebuilt = 0;
-    if (sorter_valid(sorter)) rebuilt = sorter; else if (sorter > 0) return LIBBSC_DATA_CORRUPT;
-    if (coder >= 1 && coder <= 3) rebuilt += coder << 5; else if (coder > 0) return LIBBSC_DATA_CORRUPT;
-    if (lzpMin != 0 || lzpHash != 0) {
-        if (lzpMin < 4 || lzpMin > 255) return LIBBSC_DATA_CORRUPT;
-        if (lzpHash < 10 || lzpHash > 28) return LIBBSC_DATA_CORRUPT;
-        rebuilt += (lzpMin << 8) + (lzpHash << 16);
-    }
-    if (rebuilt != mode) return LIBBSC_DATA_CORRUPT;
-    if (blockSize < LIBBSC_HEADER_SIZE || blockSize > LIBBSC_HEADER_SIZE + dataSize) return LIBBSC_DATA_CORRUPT;
-    if (index < 0 || index > dataSize) return LIBBSC_DATA_CORRUPT;
-    if (pBlockSize) *pBlockSize = blockSize;
-    if (pDataSize) *pDataSize = dataSize;
+    const int dataSize = H.data_size;
+    // the LZP stream, then the data after it: the caller's buffer is written only once the data is known to be right
+    unsigned char *lz = (unsigned char *)bsc_malloc((size_t)lzSize + (size_t)dataSize + 1);
+    if (!lz) return LIBBSC_NOT_ENOUGH_MEMORY;
+    unsigned char *data = lz + lzSize;
+    if (lzSize > 0) { CUDA_TRY(cudaMemcpyAsync(lz, d_lz, (size_t)lzSize, cudaMemcpyDeviceToHost, ctx->stream)); ctx->sync(); }
+    int r = lzp_host::decompress(lz, lzSize, data, dataSize, H.mode.lzp_hash(), H.mode.lzp_min());
+    if (r >= 0) r = (r == dataSize && H.adler_data == host_adler32(data, (size_t)dataSize)) ? LIBBSC_NO_ERROR : LIBBSC_DATA_CORRUPT;
+    if (r == LIBBSC_NO_ERROR && dataSize > 0) memcpy(output, data, (size_t)dataSize);
+    bsc_free(lz);
+    return r;
+}
+
+// The last step, once the inverse sort left lzSize bytes at d_T: undo LZP on the host, or check the length and the data Adler-32 and
+// copy the data to `output` (null on the device-resident entry point).  `output` is written only once the data is known to be right.
+int deliver(Ctx *ctx, const BlockHeader &H, const u8 *d_T, int lzSize, unsigned char *output)
+{
+    if (H.mode.has_lzp()) return undo_lzp_host(ctx, H, d_T, lzSize, output);
+    if (lzSize != H.data_size || H.adler_data != stage_adler32(ctx, d_T, H.data_size)) return LIBBSC_DATA_CORRUPT;
+    if (output && H.data_size > 0) { CUDA_TRY(cudaMemcpyAsync(output, d_T, (size_t)H.data_size, cudaMemcpyDeviceToHost, ctx->stream)); ctx->sync(); }
     return LIBBSC_NO_ERROR;
 }
 
@@ -372,44 +480,36 @@ bool secondary_indexes_out_of_range(Ctx *ctx, const u8 *d_payload, int payload, 
     return false;
 }
 
-// bsc_decompress body once the 28-byte header `h` is on the host and the block is in HBM.
-// `lz_out` (host-pointer entry point only): blocks with an LZP stage (mode bits 8..23) are decoded up to the LZP stream, whose
-// length goes to *lz_out; the caller undoes LZP on the host (lzp_host.h) and checks length and Adler-32 of the data there.
-int decompress_dev(Ctx *ctx, const unsigned char *h, const u8 *d_block, int inputSize, u8 *d_out, int outputSize, int features, int *lz_out = nullptr)
+// bsc_decompress of the block at d_block on a context's arena: the inverse BWT in the arena, ST3..ST8 in a shared slab.  The data lands
+// at d_out, and in `output` for host callers.  The device-resident entry point passes no `output`: LZP stays on the host side of the
+// boundary.
+int decompress_dev(Ctx *ctx, const BlockHeader &H, const u8 *d_block, u8 *d_out, unsigned char *output, int features)
 {
-    int blockSize = 0, dataSize = 0;
-    int info = block_info_host(h, inputSize, &blockSize, &dataSize);
-    if (info != LIBBSC_NO_ERROR) return info;
-    if (inputSize < blockSize || outputSize < dataSize) return LIBBSC_UNEXPECTED_EOB;
-    const int payload = blockSize - LIBBSC_HEADER_SIZE;
-    if (get32(h + 20) != stage_adler32(ctx, d_block + LIBBSC_HEADER_SIZE, payload)) return LIBBSC_DATA_CORRUPT;
-    const int mode = (int)get32(h + 8);
-    if (mode == 0) {
+    const u8 *d_payload = d_block + LIBBSC_HEADER_SIZE;
+    if (H.adler_payload != stage_adler32(ctx, d_payload, H.payload())) return LIBBSC_DATA_CORRUPT;
+    if (H.mode.word == 0) {
         // A stored block carries exactly dataSize payload bytes (bsc_store, libbsc.cpp:68-81).  The reference copies dataSize bytes
         // whatever blockSize says (libbsc.cpp:550-555), reading past a shorter block; here such a header is corrupt.  Like the reference,
         // the data Adler-32 of a stored block is not checked: the payload Adler-32 above covers the same bytes.
-        if (payload != dataSize) return LIBBSC_DATA_CORRUPT;
-        if (dataSize > 0) CUDA_TRY(cudaMemcpyAsync(d_out, d_block + LIBBSC_HEADER_SIZE, (size_t)dataSize, cudaMemcpyDeviceToDevice, ctx->stream));
+        if (H.payload() != H.data_size) return LIBBSC_DATA_CORRUPT;
+        if (H.data_size > 0) CUDA_TRY(cudaMemcpyAsync(d_out, d_payload, (size_t)H.data_size, cudaMemcpyDeviceToDevice, ctx->stream));
         ctx->sync();
+        if (output && H.data_size > 0) { CUDA_TRY(cudaMemcpyAsync(output, d_out, (size_t)H.data_size, cudaMemcpyDeviceToHost, ctx->stream)); ctx->sync(); }
         return LIBBSC_NO_ERROR;
     }
-    const bool lzp = mode != (mode & 0xff);
-    if (lzp && !lz_out) return LIBBSC_NOT_SUPPORTED;                     // device-resident API: LZP stays on the host side of the boundary
-    const int index = (int)get32(h + 12); const u32 adler_data = get32(h + 16);
-    const int coder = (mode >> 5) & 7, sorter = mode & 0x1f;
-    if (payload < 1) return LIBBSC_DATA_CORRUPT;
-
-    int lzSize = stage_coder_decompress(ctx, d_block + LIBBSC_HEADER_SIZE, payload, d_out, dataSize, coder, features);
+    if (H.mode.has_lzp() && !output) return LIBBSC_NOT_SUPPORTED;
+    const int lzSize = decode_coder(ctx, H, d_payload, d_out, features);
     if (lzSize < 0) return lzSize;
+    const int sorter = H.mode.sorter();
     if (!sorter_valid(sorter)) return LIBBSC_DATA_CORRUPT;               // sorter field 0 with a coder: libbsc.cpp:593, after the coder stage
-    if (sorter == 1 && secondary_indexes_out_of_range(ctx, d_block + LIBBSC_HEADER_SIZE, payload, lzSize, index)) return LIBBSC_BAD_PARAMETER;
     int r;
-    if (sorter == 1) r = stage_bwt_decode(ctx, d_out, lzSize, index);
-    else { ScratchLease lease(ctx, need_st_decode((size_t)lzSize)); r = stage_st_decode(ctx, d_out, lzSize, sorter, index); }   // libbsc.cpp:584-589
+    if (sorter == 1) {
+        if (secondary_indexes_out_of_range(ctx, d_payload, H.payload(), lzSize, H.index)) return LIBBSC_BAD_PARAMETER;
+        r = stage_bwt_decode(ctx, d_out, lzSize, H.index);
+    }
+    else { ScratchLease lease(ctx, need_st_decode((size_t)lzSize)); r = stage_st_decode(ctx, d_out, lzSize, sorter, H.index); }   // libbsc.cpp:584-589
     if (r < 0) return r;
-    if (lzp) { *lz_out = lzSize; return LIBBSC_NO_ERROR; }
-    if (lzSize != dataSize) return LIBBSC_DATA_CORRUPT;
-    return adler_data == stage_adler32(ctx, d_out, dataSize) ? LIBBSC_NO_ERROR : LIBBSC_DATA_CORRUPT;
+    return deliver(ctx, H, d_out, lzSize, output);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -452,26 +552,6 @@ size_t large_st_region(size_t n) { return std::max(st_decode_lean_bytes(n), alig
 size_t large_st_arena(size_t n) { return align_up(n + 128 + 256, 256) + align_up(large_st_region(n), 256); }
 size_t large_st_bound(size_t n) { return 26 * n + n / 2 + LARGE_FIXED; }
 
-// run `body(ctx)` on a context of its own, destroyed afterwards so that none of its HBM outlives the call
-template <class F> int with_own_ctx(F body)
-{
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) { cudaGetLastError(); return LIBBSC_GPU_NOT_SUPPORTED; }
-    Ctx *c = nullptr;
-    try { c = ctx_new(dev, nullptr, true); }
-    catch (const CudaFail &f) { return map_failure(f); }
-    catch (...) { cudaGetLastError(); return LIBBSC_GPU_ERROR; }
-    int r;
-    try { r = body(c); }
-    catch (const CudaFail &f) { r = map_failure(f); }
-    catch (const std::bad_alloc &) { r = LIBBSC_NOT_ENOUGH_MEMORY; }
-    catch (...) { r = LIBBSC_GPU_ERROR; }
-    cudaStreamSynchronize(c->stream); cudaGetLastError();
-    { std::lock_guard<std::mutex> lk(g_pool_mutex); g_launches_retired += c->kernels_launched; }
-    ctx_delete(c);
-    return r;
-}
-
 // In-place bsc_compress of a block of n > 1 GiB bytes with the BWT sorter (libbsc.cpp:124-210).
 int compress_large(unsigned char *data, int n, int lzpHashSize, int lzpMinLen, int coder, int features)
 {
@@ -479,86 +559,92 @@ int compress_large(unsigned char *data, int n, int lzpHashSize, int lzpMinLen, i
     if (cudaMemGetInfo(&fr, &total) != cudaSuccess) { cudaGetLastError(); return LIBBSC_GPU_NOT_SUPPORTED; }
     if (fr < large_bound((size_t)n)) return LIBBSC_GPU_NOT_ENOUGH_MEMORY;
 
-    int m = n, mode_bits = 0; u32 adler_orig = 0;          // m: bytes that go through the sort and the coder
-    unsigned char *lzbuf = nullptr;
-    if (lzpMinLen != 0) {                                   // libbsc.cpp:139-154: LZP on the host, not in place
-        lzbuf = (unsigned char *)bsc_malloc((size_t)n + 64);
-        if (!lzbuf) return LIBBSC_NOT_ENOUGH_MEMORY;
-        const int lzSize = lzp_host::compress(data, lzbuf, n, lzpHashSize, lzpMinLen, (features & LIBBSC_FEATURE_MULTITHREADING) != 0);
-        if (lzSize >= 0) { m = lzSize; mode_bits = (lzpMinLen << 8) | (lzpHashSize << 16); adler_orig = host_adler32(data, (size_t)n); }
-        else { bsc_free(lzbuf); lzbuf = nullptr; }         // LZP did not shrink the block: continue without it (mode &= 0xff)
-    }
-    const unsigned char *src = lzbuf ? lzbuf : data;
-    const int r = with_own_ctx([&](Ctx *ctx) {
+    LzpPass lz;
+    const int e = lz.run(data, n, lzpHashSize, lzpMinLen, features);
+    if (e != LIBBSC_NO_ERROR) return e;
+    const unsigned char *src = lz.stream ? lz.stream : data;
+    const int m = lz.stream ? lz.size : n;                  // bytes that go through the sort and the coder
+    return with_own_ctx([&](Ctx *ctx) {
         Arena &A = ctx->arena;
         A.reserve(large_arena((size_t)n));
         u8 *d_blk = A.get<u8>((size_t)m + 64);
         CUDA_TRY(cudaMemcpyAsync(d_blk, src, (size_t)m, cudaMemcpyHostToDevice, ctx->stream));
-        const u32 adler_data = lzbuf ? adler_orig : stage_adler32(ctx, d_blk, m);
+        BlockHeader H;
+        H.data_size = n;
+        H.mode = Mode::of(1, coder, lz.hash, lz.min);
+        H.adler_data = lz.stream ? lz.adler_orig : stage_adler32(ctx, d_blk, m);
         // the sort may use the whole region after the block (less a margin for the arena's rounding): batches of about n / 64 entries
         const u32 B = bwt_batch_entries((u32)m, (long long)(A.cap - A.used) - (16ll << 20));
         int indexes[256]; unsigned char num_indexes = 0;
-        const int index = stage_bwt_encode_batched(ctx, d_blk, m, &num_indexes, indexes, B);
-        if (index < 0) return index;
+        H.index = stage_bwt_encode_batched(ctx, d_blk, m, &num_indexes, indexes, B);
+        if (H.index < 0) return H.index;
         u8 *d_out = A.get<u8>((size_t)m + 4096) + 4;       // payload (offset 28) lands 16-byte aligned
         const int result = stage_coder_compress(ctx, d_blk, d_out + LIBBSC_HEADER_SIZE, m, coder, features);
-        if (result == LIBBSC_NOT_SUPPORTED) return result;
-        if (result < 0 || result + 1 + 4 * num_indexes >= n) return LIBBSC_NOT_COMPRESSIBLE;     // libbsc.cpp:188-191
-        const int size = finish_dev(ctx, d_out, result, num_indexes, indexes, n, 1 | (coder << 5) | mode_bits, index, adler_data);
+        const int size = finish_dev(ctx, d_out, result, num_indexes, indexes, H);
+        if (size < 0) return size;
         CUDA_TRY(cudaMemcpyAsync(data, d_out, (size_t)size, cudaMemcpyDeviceToHost, ctx->stream));
         ctx->sync();
         return size;
     });
-    if (lzbuf) bsc_free(lzbuf);
-    return r;
-}
-
-// libbsc.cpp:599-613: undo the LZP stage of a block (header h) on the host, from the lzSize-byte LZP stream at d_lz
-int undo_lzp_host(Ctx *ctx, const unsigned char *h, const u8 *d_lz, int lzSize, unsigned char *output, int dataSize)
-{
-    const int mode = (int)get32(h + 8);
-    // the LZP stream, then the data after it: the caller's buffer is written only once the data is known to be right
-    unsigned char *lz = (unsigned char *)bsc_malloc((size_t)lzSize + (size_t)dataSize + 1);
-    if (!lz) return LIBBSC_NOT_ENOUGH_MEMORY;
-    unsigned char *data = lz + lzSize;
-    if (lzSize > 0) { CUDA_TRY(cudaMemcpyAsync(lz, d_lz, (size_t)lzSize, cudaMemcpyDeviceToHost, ctx->stream)); ctx->sync(); }
-    int r = lzp_host::decompress(lz, lzSize, data, dataSize, (mode >> 16) & 0xff, (mode >> 8) & 0xff);
-    if (r >= 0) r = (r == dataSize && get32(h + 16) == host_adler32(data, (size_t)dataSize)) ? LIBBSC_NO_ERROR : LIBBSC_DATA_CORRUPT;
-    if (r == LIBBSC_NO_ERROR && dataSize > 0) memcpy(output, data, (size_t)dataSize);
-    bsc_free(lz);
-    return r;
 }
 
 // bsc_decompress of a block with block sorter 3..8 whose data size is above 1 GiB (large_st_arena above).  The caller checked the header
-// (block_info_host) and the sizes.  The caller's buffer is written only on success.
-int decompress_large_st(const unsigned char *input, const unsigned char *h, int blockSize, int dataSize, unsigned char *output, int features)
+// and the sizes.  The caller's buffer is written only on success.
+int decompress_large_st(const unsigned char *input, const BlockHeader &H, unsigned char *output, int features)
 {
     size_t fr = 0, total = 0;
     if (cudaMemGetInfo(&fr, &total) != cudaSuccess) { cudaGetLastError(); return LIBBSC_GPU_NOT_SUPPORTED; }
-    if (fr < large_st_bound((size_t)dataSize)) return LIBBSC_GPU_NOT_ENOUGH_MEMORY;
+    if (fr < large_st_bound((size_t)H.data_size)) return LIBBSC_GPU_NOT_ENOUGH_MEMORY;
     return with_own_ctx([&](Ctx *ctx) {
         Arena &A = ctx->arena;
-        A.reserve(large_st_arena((size_t)dataSize));
-        u8 *d_L = A.get<u8>((size_t)dataSize + 128);
-        const size_t full = A.cap, blk = align_up((size_t)blockSize + 128, 256);
+        A.reserve(large_st_arena((size_t)H.data_size));
+        u8 *d_L = A.get<u8>((size_t)H.data_size + 128);
+        const size_t full = A.cap, blk = align_up((size_t)H.block_size + 128, 256);
         u8 *d_blk = A.base + full - blk + 4;                 // the top end of the region; payload (offset 28) lands 16-byte aligned
-        CUDA_TRY(cudaMemcpyAsync(d_blk, input, (size_t)blockSize, cudaMemcpyHostToDevice, ctx->stream));
-        CUDA_TRY(cudaMemsetAsync(d_blk + blockSize, 0, 64, ctx->stream));
-        const int payload = blockSize - LIBBSC_HEADER_SIZE, mode = (int)get32(h + 8), index = (int)get32(h + 12);
-        if (payload < 1) return LIBBSC_DATA_CORRUPT;
-        if (get32(h + 20) != stage_adler32(ctx, d_blk + LIBBSC_HEADER_SIZE, payload)) return LIBBSC_DATA_CORRUPT;
+        CUDA_TRY(cudaMemcpyAsync(d_blk, input, (size_t)H.block_size, cudaMemcpyHostToDevice, ctx->stream));
+        CUDA_TRY(cudaMemsetAsync(d_blk + H.block_size, 0, 64, ctx->stream));
+        const u8 *d_payload = d_blk + LIBBSC_HEADER_SIZE;
+        if (H.adler_payload != stage_adler32(ctx, d_payload, H.payload())) return LIBBSC_DATA_CORRUPT;
         A.cap = full - blk;                                  // the coder stage stays below the block
-        const int lzSize = stage_coder_decompress(ctx, d_blk + LIBBSC_HEADER_SIZE, payload, d_L, dataSize, (mode >> 5) & 7, features);
+        const int lzSize = decode_coder(ctx, H, d_payload, d_L, features);
         A.cap = full;
         if (lzSize < 0) return lzSize;
         u8 *d_T = nullptr;                                   // the block is dead: the inverse ST takes the whole region after L
-        const int r = stage_st_decode_lean(ctx, d_L, lzSize, mode & 0x1f, index, &d_T);
+        const int r = stage_st_decode_lean(ctx, d_L, lzSize, H.mode.sorter(), H.index, &d_T);
         if (r < 0) return r;
-        if (mode != (mode & 0xff)) return undo_lzp_host(ctx, h, d_T, lzSize, output, dataSize);
-        if (lzSize != dataSize || get32(h + 16) != stage_adler32(ctx, d_T, dataSize)) return LIBBSC_DATA_CORRUPT;
-        CUDA_TRY(cudaMemcpyAsync(output, d_T, (size_t)dataSize, cudaMemcpyDeviceToHost, ctx->stream));
-        ctx->sync();
-        return LIBBSC_NO_ERROR;
+        return deliver(ctx, H, d_T, lzSize, output);
+    });
+}
+
+// ---------------------------------------------------------------------------------------------
+// host-pointer stage entry points: the data goes in, through one stage on the device, and back when the stage succeeds
+// ---------------------------------------------------------------------------------------------
+// T (n bytes) through `stage(ctx, d_T)`, which works in place; T is written back when the stage returns r >= 0.
+template <class F> int stage_in_place(unsigned char *T, int n, size_t reserve, F stage)
+{
+    return with_ctx([&](Ctx *ctx) {
+        ctx->arena.reserve(reserve);
+        u8 *d = ctx->arena.get<u8>((size_t)n + 64);
+        if (n > 0) CUDA_TRY(cudaMemcpyAsync(d, T, (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
+        const int r = stage(ctx, d);
+        if (r >= 0 && n > 0) { CUDA_TRY(cudaMemcpyAsync(T, d, (size_t)n, cudaMemcpyDeviceToHost, ctx->stream)); ctx->sync(); }
+        return r;
+    });
+}
+
+// inSize bytes at `input` through `stage(ctx, d_in, d_out)` into a device buffer of out_room bytes; the r > 0 bytes the stage returns
+// go to `output`.  The decoders (`pad`) read ahead: 64 zero bytes follow their input.
+template <class F> int stage_to_output(const unsigned char *input, int inSize, unsigned char *output, size_t out_room, size_t reserve, bool pad, F stage)
+{
+    return with_ctx([&](Ctx *ctx) {
+        ctx->arena.reserve(reserve);
+        u8 *d_in = ctx->arena.get<u8>((size_t)inSize + (pad ? 128 : 64));
+        u8 *d_out = ctx->arena.get<u8>(out_room);
+        CUDA_TRY(cudaMemcpyAsync(d_in, input, (size_t)inSize, cudaMemcpyHostToDevice, ctx->stream));
+        if (pad) CUDA_TRY(cudaMemsetAsync(d_in + inSize, 0, 64, ctx->stream));
+        const int r = stage(ctx, d_in, d_out);
+        if (r > 0) { CUDA_TRY(cudaMemcpyAsync(output, d_out, (size_t)r, cudaMemcpyDeviceToHost, ctx->stream)); ctx->sync(); }
+        return r;
     });
 }
 
@@ -587,7 +673,6 @@ int bsc_init_full(int features, void *(*malloc_fn)(size_t), void *(*zero_malloc_
     setenv("CUDA_DEVICE_MAX_CONNECTIONS", "32", 0);
     int count = 0;
     if (cudaGetDeviceCount(&count) != cudaSuccess || count < 1) { cudaGetLastError(); return LIBBSC_GPU_NOT_SUPPORTED; }
-    g_features = features; g_initialised = true;
     return LIBBSC_NO_ERROR;
 }
 int bsc_init(int features) { return bsc_init_full(features, nullptr, nullptr, nullptr); }
@@ -617,24 +702,26 @@ int bsc_store(const unsigned char *input, unsigned char *output, int n, int feat
     if (n < 0) return LIBBSC_BAD_PARAMETER;
     unsigned int a = bsc_adler32(input, n, features);
     memmove(output + LIBBSC_HEADER_SIZE, input, (size_t)n);
-    put32(output, (u32)(n + LIBBSC_HEADER_SIZE)); put32(output + 4, (u32)n); put32(output + 8, 0); put32(output + 12, 0);
-    put32(output + 16, a); put32(output + 20, a); put32(output + 24, host_adler32(output, 24));
+    BlockHeader{n + LIBBSC_HEADER_SIZE, n, Mode{0}, 0, a, a}.write(output);
     return n + LIBBSC_HEADER_SIZE;
 }
 
 int bsc_block_info(const unsigned char *blockHeader, int headerSize, int *pBlockSize, int *pDataSize, int features)
 {
     (void)features;
-    return block_info_host(blockHeader, headerSize, pBlockSize, pDataSize);
+    BlockHeader H;
+    const int r = H.read(blockHeader, headerSize);
+    if (r != LIBBSC_NO_ERROR) return r;
+    if (pBlockSize) *pBlockSize = H.block_size;
+    if (pDataSize) *pDataSize = H.data_size;
+    return LIBBSC_NO_ERROR;
 }
 
 int bsc_compress(const unsigned char *input, unsigned char *output, int n, int lzpHashSize, int lzpMinLen, int blockSorter, int coder, int features)
 {
-    if (!sorter_valid(blockSorter)) return LIBBSC_BAD_PARAMETER;
-    if (coder < 1 || coder > 3) return LIBBSC_BAD_PARAMETER;
+    if (!sorter_valid(blockSorter) || !coder_valid(coder)) return LIBBSC_BAD_PARAMETER;
     if (lzpMinLen != 0 || lzpHashSize != 0) {
-        if (lzpMinLen < 4 || lzpMinLen > 255) return LIBBSC_BAD_PARAMETER;
-        if (lzpHashSize < 10 || lzpHashSize > 28) return LIBBSC_BAD_PARAMETER;
+        if (!lzp_valid(lzpHashSize, lzpMinLen)) return LIBBSC_BAD_PARAMETER;
         // The LZP stage runs on the host (lzp_host.h: all five x86-64 variants of the reference; north star: libbsc/lzp stays on the host).
         if (!lzp_host::supported(lzpHashSize, lzpMinLen)) return LIBBSC_NOT_SUPPORTED;
     }
@@ -644,60 +731,40 @@ int bsc_compress(const unsigned char *input, unsigned char *output, int n, int l
     // In place only: compress_large works on its argument in place.  Out of place, blocks above 1 GiB were refused above, and below it a
     // lowered routing threshold (tests) keeps them on the pooled path.
     if (inplace && n > large_route_n()) return blockSorter == 1 ? compress_large(output, n, lzpHashSize, lzpMinLen, coder, features) : LIBBSC_NOT_SUPPORTED;
-    if (lzpMinLen != 0) {                                   // libbsc.cpp:264-276
-        unsigned char *lzbuf = (unsigned char *)bsc_malloc((size_t)n + 64);
-        if (!lzbuf) return LIBBSC_NOT_ENOUGH_MEMORY;
-        const int lzSize = lzp_host::compress(input, lzbuf, n, lzpHashSize, lzpMinLen, (features & LIBBSC_FEATURE_MULTITHREADING) != 0);
-        if (lzSize >= 0) {
-            const LzpInfo lz = {n, host_adler32(input, (size_t)n), (lzpMinLen << 8) | (lzpHashSize << 16)};
-            int r = with_ctx([&](Ctx *ctx) {
-                ctx->arena.reserve(host_compress_bytes(n));
-                u8 *d_in = ctx->arena.get<u8>((size_t)lzSize + 64);
-                u8 *d_out = ctx->arena.get<u8>((size_t)n + 4096) + 4;
-                if (lzSize > 0) CUDA_TRY(cudaMemcpyAsync(d_in, lzbuf, (size_t)lzSize, cudaMemcpyHostToDevice, ctx->stream));
-                int rr = compress_dev(ctx, d_in, lzSize, d_out, blockSorter, coder, features, inplace, &lz);
-                if (rr > 0) { CUDA_TRY(cudaMemcpyAsync(output, d_out, (size_t)rr, cudaMemcpyDeviceToHost, ctx->stream)); ctx->sync(); }
-                return rr;
-            });
-            bsc_free(lzbuf);
-            if (r == LIBBSC_NOT_COMPRESSIBLE && !inplace) return bsc_store(input, output, n, features);
-            return r;
-        }
-        bsc_free(lzbuf);                                    // LZP did not shrink the block: continue without it (mode &= 0xff)
-    }
-    return with_ctx([&](Ctx *ctx) {
+    LzpPass lz;
+    int r = lz.run(input, n, lzpHashSize, lzpMinLen, features);
+    if (r != LIBBSC_NO_ERROR) return r;
+    const unsigned char *src = lz.stream ? lz.stream : input;
+    const int m = lz.stream ? lz.size : n;
+    r = with_ctx([&](Ctx *ctx) {
         ctx->arena.reserve(host_compress_bytes(n));
-        u8 *d_in = ctx->arena.get<u8>((size_t)n + 64);
+        u8 *d_in = ctx->arena.get<u8>((size_t)m + 64);
         u8 *d_out = ctx->arena.get<u8>((size_t)n + 4096) + 4;      // payload (offset 28) lands 16-byte aligned
-        CUDA_TRY(cudaMemcpyAsync(d_in, input, (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
-        int r = compress_dev(ctx, d_in, n, d_out, blockSorter, coder, features, inplace);
-        if (r > 0) { CUDA_TRY(cudaMemcpyAsync(output, d_out, (size_t)r, cudaMemcpyDeviceToHost, ctx->stream)); ctx->sync(); }
-        return r;
+        if (m > 0) CUDA_TRY(cudaMemcpyAsync(d_in, src, (size_t)m, cudaMemcpyHostToDevice, ctx->stream));
+        const int size = compress_dev(ctx, d_in, m, d_out, blockSorter, coder, features, inplace, lz.stream ? &lz : nullptr);
+        if (size > 0) { CUDA_TRY(cudaMemcpyAsync(output, d_out, (size_t)size, cudaMemcpyDeviceToHost, ctx->stream)); ctx->sync(); }
+        return size;
     });
+    if (r == LIBBSC_NOT_COMPRESSIBLE && lz.stream && !inplace) return bsc_store(input, output, n, features);
+    return r;
 }
 
 int bsc_decompress(const unsigned char *input, int inputSize, unsigned char *output, int outputSize, int features)
 {
-    int blockSize = 0, dataSize = 0;
-    int info = block_info_host(input, inputSize, &blockSize, &dataSize);
+    BlockHeader H;
+    const int info = H.read(input, inputSize);
     if (info != LIBBSC_NO_ERROR) return info;
-    if (inputSize < blockSize || outputSize < dataSize) return LIBBSC_UNEXPECTED_EOB;
-    unsigned char h[LIBBSC_HEADER_SIZE]; memcpy(h, input, LIBBSC_HEADER_SIZE);
-    const bool large = dataSize > large_route_n();
-    if (large && (get32(h + 8) & 0x1f) >= 3) return decompress_large_st(input, h, blockSize, dataSize, output, features);
-    // Above 1 GiB (BWT and stored blocks): about 10.7 n + 28 MB (large_bound holds it), on a context of its own that does not keep it after the call.
+    if (inputSize < H.block_size || outputSize < H.data_size) return LIBBSC_UNEXPECTED_EOB;
+    const bool large = H.data_size > large_route_n();
+    if (large && H.mode.sorter() >= 3) return decompress_large_st(input, H, output, features);
+    // Above 1 GiB (BWT and stored blocks): on a context of its own that does not keep its HBM after the call.
     auto body = [&](Ctx *ctx) {
-        ctx->arena.reserve(Arena::bytes_for<u8>((size_t)blockSize + 128) + Arena::bytes_for<u8>((size_t)dataSize + 128)
-                           + std::max(need_coder((size_t)dataSize), bwt_decode_bytes((u32)dataSize)));     // coder stage, then the inverse BWT in the same space
-        u8 *d_blk = ctx->arena.get<u8>((size_t)blockSize + 128) + 4;
-        u8 *d_out = ctx->arena.get<u8>((size_t)dataSize + 128);
-        CUDA_TRY(cudaMemcpyAsync(d_blk, input, (size_t)blockSize, cudaMemcpyHostToDevice, ctx->stream));
-        CUDA_TRY(cudaMemsetAsync(d_blk + blockSize, 0, 64, ctx->stream));
-        int lzSize = -1;
-        int r = decompress_dev(ctx, h, d_blk, blockSize, d_out, dataSize, features, &lzSize);
-        if (r == LIBBSC_NO_ERROR && lzSize >= 0) return undo_lzp_host(ctx, h, d_out, lzSize, output, dataSize);
-        if (r == LIBBSC_NO_ERROR && dataSize > 0) { CUDA_TRY(cudaMemcpyAsync(output, d_out, (size_t)dataSize, cudaMemcpyDeviceToHost, ctx->stream)); ctx->sync(); }
-        return r;
+        ctx->arena.reserve(host_decompress_bytes((size_t)H.block_size, (size_t)H.data_size));
+        u8 *d_blk = ctx->arena.get<u8>((size_t)H.block_size + 128) + 4;
+        u8 *d_out = ctx->arena.get<u8>((size_t)H.data_size + 128);
+        CUDA_TRY(cudaMemcpyAsync(d_blk, input, (size_t)H.block_size, cudaMemcpyHostToDevice, ctx->stream));
+        CUDA_TRY(cudaMemsetAsync(d_blk + H.block_size, 0, 64, ctx->stream));
+        return decompress_dev(ctx, H, d_blk, d_out, output, features);
     };
     return large ? with_own_ctx(body) : with_ctx(body);
 }
@@ -706,14 +773,7 @@ int bsc_bwt_encode(unsigned char *T, int n, unsigned char *num_indexes, int *ind
 {
     (void)features;
     if (T == nullptr || n < 0) return LIBBSC_BAD_PARAMETER;
-    return with_ctx([&](Ctx *ctx) {
-        ctx->arena.reserve((size_t)n + 4096);
-        u8 *d = ctx->arena.get<u8>((size_t)n + 64);
-        if (n > 0) CUDA_TRY(cudaMemcpyAsync(d, T, (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
-        int r = bwt_encode_leased(ctx, d, n, num_indexes, indexes);
-        if (r >= 0 && n > 0) { CUDA_TRY(cudaMemcpyAsync(T, d, (size_t)n, cudaMemcpyDeviceToHost, ctx->stream)); ctx->sync(); }
-        return r;
-    });
+    return stage_in_place(T, n, (size_t)n + 4096, [&](Ctx *ctx, u8 *d) { return bwt_encode_leased(ctx, d, n, num_indexes, indexes); });
 }
 
 int bsc_bwt_decode(unsigned char *T, int n, int index, unsigned char num_indexes, int *indexes, int features)
@@ -721,31 +781,17 @@ int bsc_bwt_decode(unsigned char *T, int n, int index, unsigned char num_indexes
     (void)num_indexes; (void)indexes; (void)features;    // secondary indexes are CPU accelerators only (bwt.cpp:263 ignores them on the GPU too)
     if (T == nullptr || n < 0 || index <= 0 || index > n) return LIBBSC_BAD_PARAMETER;
     if (n <= 1) return LIBBSC_NO_ERROR;
-    return with_ctx([&](Ctx *ctx) {
-        ctx->arena.reserve(Arena::bytes_for<u8>((size_t)n + 64) + bwt_decode_bytes((u32)n));
-        u8 *d = ctx->arena.get<u8>((size_t)n + 64);
-        CUDA_TRY(cudaMemcpyAsync(d, T, (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
-        int r = stage_bwt_decode(ctx, d, n, index);
-        if (r == 0) { CUDA_TRY(cudaMemcpyAsync(T, d, (size_t)n, cudaMemcpyDeviceToHost, ctx->stream)); ctx->sync(); }
-        return r;
-    });
+    return stage_in_place(T, n, Arena::bytes_for<u8>((size_t)n + 64) + bwt_decode_bytes((u32)n),
+                          [&](Ctx *ctx, u8 *d) { return stage_bwt_decode(ctx, d, n, index); });
 }
 
 int bsc_st_encode(unsigned char *T, int n, int k, int features)
 {
     (void)features;
     if (T == nullptr || n < 0) return LIBBSC_BAD_PARAMETER;
-    if (k < 3 || k > 8) return LIBBSC_BAD_PARAMETER;
+    if (!st_order_valid(k)) return LIBBSC_BAD_PARAMETER;
     if (n <= 1) return 0;
-    return with_ctx([&](Ctx *ctx) {
-        ctx->arena.reserve((size_t)n + 4096);
-        u8 *d = ctx->arena.get<u8>((size_t)n + 64);
-        CUDA_TRY(cudaMemcpyAsync(d, T, (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
-        ScratchLease lease(ctx, need_st_encode(n));
-        int r = stage_st_encode(ctx, d, n, k);
-        if (r >= 0) { CUDA_TRY(cudaMemcpyAsync(T, d, (size_t)n, cudaMemcpyDeviceToHost, ctx->stream)); ctx->sync(); }
-        return r;
-    });
+    return stage_in_place(T, n, (size_t)n + 4096, [&](Ctx *ctx, u8 *d) { ScratchLease lease(ctx, need_st_encode(n)); return stage_st_encode(ctx, d, n, k); });
 }
 
 int bsc_st_decode(unsigned char *T, int n, int k, int index, int features)
@@ -753,49 +799,27 @@ int bsc_st_decode(unsigned char *T, int n, int k, int index, int features)
     (void)features;
     if (T == nullptr || n < 0) return LIBBSC_BAD_PARAMETER;       // st.cpp:1493-1496
     if (index < 0 || index >= n) return LIBBSC_BAD_PARAMETER;
-    if (k < 3 || k > 8) return LIBBSC_BAD_PARAMETER;
+    if (!st_order_valid(k)) return LIBBSC_BAD_PARAMETER;
     if (n <= 1) return LIBBSC_NO_ERROR;
-    return with_ctx([&](Ctx *ctx) {
-        ctx->arena.reserve((size_t)n + 4096);
-        u8 *d = ctx->arena.get<u8>((size_t)n + 64);
-        CUDA_TRY(cudaMemcpyAsync(d, T, (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
-        ScratchLease lease(ctx, need_st_decode(n));
-        int r = stage_st_decode(ctx, d, n, k, index);
-        if (r == 0) { CUDA_TRY(cudaMemcpyAsync(T, d, (size_t)n, cudaMemcpyDeviceToHost, ctx->stream)); ctx->sync(); }
-        return r;
-    });
+    return stage_in_place(T, n, (size_t)n + 4096, [&](Ctx *ctx, u8 *d) { ScratchLease lease(ctx, need_st_decode(n)); return stage_st_decode(ctx, d, n, k, index); });
 }
 
 int bsc_coder_compress(const unsigned char *input, unsigned char *output, int n, int coder, int features)
 {
-    if (coder < 1 || coder > 3) return LIBBSC_BAD_PARAMETER;
+    if (!coder_valid(coder)) return LIBBSC_BAD_PARAMETER;
     if (n <= 0) return LIBBSC_BAD_PARAMETER;
-    return with_ctx([&](Ctx *ctx) {
-        ctx->arena.reserve(2 * (size_t)n + 16384 + need_coder(n));
-        u8 *d_in = ctx->arena.get<u8>((size_t)n + 64);
-        u8 *d_out = ctx->arena.get<u8>((size_t)n + 4096);
-        CUDA_TRY(cudaMemcpyAsync(d_in, input, (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
-        int r = stage_coder_compress(ctx, d_in, d_out, n, coder, features);
-        if (r > 0) { CUDA_TRY(cudaMemcpyAsync(output, d_out, (size_t)r, cudaMemcpyDeviceToHost, ctx->stream)); ctx->sync(); }
-        return r;
-    });
+    return stage_to_output(input, n, output, (size_t)n + 4096, 2 * (size_t)n + 16384 + need_coder(n), false,
+                           [&](Ctx *ctx, const u8 *d_in, u8 *d_out) { return stage_coder_compress(ctx, d_in, d_out, n, coder, features); });
 }
 
 // Size-aware variant used by bsc_decompress and exported for integrators.
 int bscb200_coder_decompress(const unsigned char *input, int inputSize, unsigned char *output, int outputCapacity, int coder, int features)
 {
-    if (coder < 1 || coder > 3) return LIBBSC_BAD_PARAMETER;
+    if (!coder_valid(coder)) return LIBBSC_BAD_PARAMETER;
     if (inputSize < 1 || outputCapacity < 0) return LIBBSC_BAD_PARAMETER;
-    return with_ctx([&](Ctx *ctx) {
-        ctx->arena.reserve((size_t)inputSize + (size_t)outputCapacity + 16384 + need_coder((size_t)outputCapacity));
-        u8 *d_in = ctx->arena.get<u8>((size_t)inputSize + 128);
-        u8 *d_out = ctx->arena.get<u8>((size_t)outputCapacity + 128);
-        CUDA_TRY(cudaMemcpyAsync(d_in, input, (size_t)inputSize, cudaMemcpyHostToDevice, ctx->stream));
-        CUDA_TRY(cudaMemsetAsync(d_in + inputSize, 0, 64, ctx->stream));
-        int r = stage_coder_decompress(ctx, d_in, inputSize, d_out, outputCapacity, coder, features);
-        if (r > 0) { CUDA_TRY(cudaMemcpyAsync(output, d_out, (size_t)r, cudaMemcpyDeviceToHost, ctx->stream)); ctx->sync(); }
-        return r;
-    });
+    return stage_to_output(input, inputSize, output, (size_t)outputCapacity + 128,
+                           (size_t)inputSize + (size_t)outputCapacity + 16384 + need_coder((size_t)outputCapacity), true,
+                           [&](Ctx *ctx, const u8 *d_in, u8 *d_out) { return stage_coder_decompress(ctx, d_in, inputSize, d_out, outputCapacity, coder, features); });
 }
 
 // The uncompressed size n of a QLFC stream = its first 32 range-coded bits, each with p = 1/2 (qlfc.cpp:852; rangecoder.h:203-240).
@@ -819,7 +843,7 @@ static long long qlfc_stream_size(const unsigned char *p)
 // beyond the stream's end).  Integrators that know their sizes should call bscb200_coder_decompress.
 int bsc_coder_decompress(const unsigned char *input, unsigned char *output, int coder, int features)
 {
-    if (coder < 1 || coder > 3) return LIBBSC_BAD_PARAMETER;
+    if (!coder_valid(coder)) return LIBBSC_BAD_PARAMETER;
     int nBlocks = input[0];
     long long inSize = 0, outSize = 0;
     if (nBlocks == 1) {
@@ -839,16 +863,9 @@ int bsc_coder_decompress(const unsigned char *input, unsigned char *output, int 
 static int qlfc_encode_block(int coder, const unsigned char *input, unsigned char *output, int inputSize, int outputSize)
 {
     if (inputSize <= 0 || outputSize < 0) return LIBBSC_BAD_PARAMETER;
-    return with_ctx([&](Ctx *ctx) {
-        const size_t room = (size_t)(outputSize > inputSize ? outputSize : inputSize);
-        ctx->arena.reserve(2 * room + (size_t)inputSize + 16384 + need_coder(room));
-        u8 *d_in = ctx->arena.get<u8>((size_t)inputSize + 64);
-        u8 *d_out = ctx->arena.get<u8>(room + 4096);
-        CUDA_TRY(cudaMemcpyAsync(d_in, input, (size_t)inputSize, cudaMemcpyHostToDevice, ctx->stream));
-        int r = stage_coder_compress(ctx, d_in, d_out, inputSize, coder, 0, outputSize);
-        if (r > 0) { CUDA_TRY(cudaMemcpyAsync(output, d_out, (size_t)r, cudaMemcpyDeviceToHost, ctx->stream)); ctx->sync(); }
-        return r;
-    });
+    const size_t room = (size_t)(outputSize > inputSize ? outputSize : inputSize);
+    return stage_to_output(input, inputSize, output, room + 4096, 2 * room + (size_t)inputSize + 16384 + need_coder(room), false,
+                           [&](Ctx *ctx, const u8 *d_in, u8 *d_out) { return stage_coder_compress(ctx, d_in, d_out, inputSize, coder, 0, outputSize); });
 }
 // Size-less like the reference's: n comes from the stream; the stream is taken to be at most n + 16 bytes long (what
 // bsc_qlfc_*_encode_block produces with outputSize <= inputSize; same caller contract as bsc_coder_decompress above).
@@ -858,16 +875,8 @@ static int qlfc_decode_block(int coder, const unsigned char *input, unsigned cha
     if (n < 0) return LIBBSC_DATA_CORRUPT;
     const int inSize = (int)readable_prefix(input, (size_t)n + 16);
     if (inSize < 14) return LIBBSC_UNEXPECTED_EOB;
-    return with_ctx([&](Ctx *ctx) {
-        ctx->arena.reserve((size_t)inSize + (size_t)n + 16384 + need_coder((size_t)n));
-        u8 *d_in = ctx->arena.get<u8>((size_t)inSize + 128);
-        u8 *d_out = ctx->arena.get<u8>((size_t)n + 128);
-        CUDA_TRY(cudaMemcpyAsync(d_in, input, (size_t)inSize, cudaMemcpyHostToDevice, ctx->stream));
-        CUDA_TRY(cudaMemsetAsync(d_in + inSize, 0, 64, ctx->stream));
-        int r = stage_coder_decompress(ctx, d_in, inSize, d_out, (int)n, coder, 0, true);
-        if (r > 0) { CUDA_TRY(cudaMemcpyAsync(output, d_out, (size_t)r, cudaMemcpyDeviceToHost, ctx->stream)); ctx->sync(); }
-        return r;
-    });
+    return stage_to_output(input, inSize, output, (size_t)n + 128, (size_t)inSize + (size_t)n + 16384 + need_coder((size_t)n), true,
+                           [&](Ctx *ctx, const u8 *d_in, u8 *d_out) { return stage_coder_decompress(ctx, d_in, inSize, d_out, (int)n, coder, 0, true); });
 }
 int bsc_qlfc_static_encode_block(const unsigned char *input, unsigned char *output, int inputSize, int outputSize) { return qlfc_encode_block(1, input, output, inputSize, outputSize); }
 int bsc_qlfc_adaptive_encode_block(const unsigned char *input, unsigned char *output, int inputSize, int outputSize) { return qlfc_encode_block(2, input, output, inputSize, outputSize); }
@@ -881,12 +890,7 @@ void *bscb200_ctx_create(int device, void *cuda_stream)
 {
     try { return ctx_new(device, (cudaStream_t)cuda_stream, cuda_stream == nullptr); } catch (...) { cudaGetLastError(); return nullptr; }
 }
-void bscb200_ctx_destroy(void *ctx)
-{
-    Ctx *c = (Ctx *)ctx;
-    if (c) { std::lock_guard<std::mutex> lk(g_pool_mutex); g_launches_retired += c->kernels_launched; }
-    ctx_delete(c);
-}
+void bscb200_ctx_destroy(void *ctx) { ctx_delete((Ctx *)ctx); }
 int bscb200_ctx_reserve(void *ctx, long long bytes)
 {
     Ctx *c = (Ctx *)ctx;
@@ -916,7 +920,7 @@ long long bscb200_scratch_bytes(int n, int blockSorter)     /* size of one share
 // HBM that an in-place bsc_compress of a block above 1 GiB, or bsc_decompress of one, takes at most: 18 n + 256 MiB (large_bound)
 long long bscb200_inplace_bytes(int n, int blockSorter, int coder)
 {
-    if (n < 0 || n > 2146435072 || !sorter_valid(blockSorter) || coder < 1 || coder > 3) return LIBBSC_BAD_PARAMETER;
+    if (n < 0 || n > 2146435072 || !sorter_valid(blockSorter) || !coder_valid(coder)) return LIBBSC_BAD_PARAMETER;
     if (blockSorter != 1) return LIBBSC_NOT_SUPPORTED;      // no bounded sort transform
     return (long long)large_bound((size_t)n);
 }
@@ -931,7 +935,7 @@ long long bscb200_decompress_bytes(int n, int blockSorter)
 // host-only: the inverse LZP stage by itself (what bsc_decompress runs after the GPU stages), for CPU tests against the reference
 int bscb200_lzp_decompress_host(const unsigned char *input, int n, unsigned char *output, int outputCapacity, int lzpHashSize, int lzpMinLen)
 {
-    if (!input || !output || n < 0 || outputCapacity < 0 || lzpHashSize < 10 || lzpHashSize > 28 || lzpMinLen < 4 || lzpMinLen > 255) return LIBBSC_BAD_PARAMETER;
+    if (!input || !output || n < 0 || outputCapacity < 0 || !lzp_valid(lzpHashSize, lzpMinLen)) return LIBBSC_BAD_PARAMETER;
     return lzp_host::decompress(input, n, output, outputCapacity, lzpHashSize, lzpMinLen);
 }
 
@@ -939,7 +943,7 @@ int bscb200_lzp_decompress_host(const unsigned char *input, int n, unsigned char
 // reference variant is not restated (lzp_host.h)
 int bscb200_lzp_compress_host(const unsigned char *input, unsigned char *output, int n, int lzpHashSize, int lzpMinLen, int features)
 {
-    if (!input || !output || n < 0 || lzpHashSize < 10 || lzpHashSize > 28 || lzpMinLen < 4 || lzpMinLen > 255) return LIBBSC_BAD_PARAMETER;
+    if (!input || !output || n < 0 || !lzp_valid(lzpHashSize, lzpMinLen)) return LIBBSC_BAD_PARAMETER;
     if (!lzp_host::supported(lzpHashSize, lzpMinLen)) return LIBBSC_NOT_SUPPORTED;
     return lzp_host::compress(input, output, n, lzpHashSize, lzpMinLen, (features & LIBBSC_FEATURE_MULTITHREADING) != 0);
 }
@@ -955,11 +959,11 @@ void bscb200_release_pools(void)
     int cur = 0; cudaGetDevice(&cur);
     for (int d = 0; d < MAX_DEVICES; ++d) {
         std::vector<Ctx *> ctxs; std::vector<Scratch *> slabs;
-        { std::lock_guard<std::mutex> lk(g_pool_mutex); ctxs.swap(g_pool[d]); for (Ctx *c : ctxs) g_launches_retired += c->kernels_launched; }
+        { std::lock_guard<std::mutex> lk(g_pool_mutex); ctxs.swap(g_pool[d]); }
         { std::lock_guard<std::mutex> lk(g_scratch[d].m); slabs.swap(g_scratch[d].free_list); g_scratch[d].created -= (int)slabs.size(); g_scratch[d].cap = -1; }
         for (Ctx *c : ctxs) ctx_delete(c);
         if (!slabs.empty()) cudaSetDevice(d);
-        for (Scratch *s : slabs) { if (s->idle_valid) cudaEventSynchronize(s->idle); s->arena.destroy(); if (s->idle) cudaEventDestroy(s->idle); delete s; }
+        for (Scratch *s : slabs) scratch_destroy(s);
     }
     cudaSetDevice(cur); cudaGetLastError();
 }
@@ -980,11 +984,14 @@ int bscb200_decompress_device(void *ctx, const unsigned char *d_input, int input
     Ctx *c = (Ctx *)ctx;
     return guarded(c, [&]() {
         if (inputSize < LIBBSC_HEADER_SIZE) return LIBBSC_UNEXPECTED_EOB;
-        unsigned char h[LIBBSC_HEADER_SIZE];
         CUDA_TRY(cudaMemcpyAsync(c->h_mail + 64, d_input, LIBBSC_HEADER_SIZE, cudaMemcpyDeviceToHost, c->stream));
-        c->sync(); memcpy(h, c->h_mail + 64, LIBBSC_HEADER_SIZE);
+        c->sync();
         c->arena.reset(); c->arena.reserve((size_t)bscb200_workspace_bytes_decode(outputSize));   // no-op for a context that already compressed
-        return decompress_dev(c, h, d_input, inputSize, d_output, outputSize, features);
+        BlockHeader H;
+        const int info = H.read((const unsigned char *)(c->h_mail + 64), inputSize);
+        if (info != LIBBSC_NO_ERROR) return info;
+        if (inputSize < H.block_size || outputSize < H.data_size) return LIBBSC_UNEXPECTED_EOB;
+        return decompress_dev(c, H, d_input, d_output, nullptr, features);
     });
 }
 int bscb200_bwt_encode_device(void *ctx, unsigned char *d_T, int n, unsigned char *num_indexes, int *indexes)
@@ -1001,25 +1008,25 @@ int bscb200_bwt_decode_device(void *ctx, unsigned char *d_T, int n, int index)
 int bscb200_st_encode_device(void *ctx, unsigned char *d_T, int n, int k)
 {
     Ctx *c = (Ctx *)ctx;
-    if (d_T == nullptr || n < 0 || k < 3 || k > 8) return LIBBSC_BAD_PARAMETER;
+    if (d_T == nullptr || n < 0 || !st_order_valid(k)) return LIBBSC_BAD_PARAMETER;
     return guarded(c, [&]() { c->arena.reset(); ScratchLease lease(c, need_st_encode((size_t)n)); return stage_st_encode(c, d_T, n, k); });
 }
 int bscb200_st_decode_device(void *ctx, unsigned char *d_T, int n, int k, int index)
 {
     Ctx *c = (Ctx *)ctx;
-    if (d_T == nullptr || n < 0 || index < 0 || index >= n || k < 3 || k > 8) return LIBBSC_BAD_PARAMETER;     // st.cpp:1493-1495
+    if (d_T == nullptr || n < 0 || index < 0 || index >= n || !st_order_valid(k)) return LIBBSC_BAD_PARAMETER;     // st.cpp:1493-1495
     return guarded(c, [&]() { c->arena.reset(); ScratchLease lease(c, need_st_decode((size_t)n)); int r = stage_st_decode(c, d_T, n, k, index); c->sync(); return r; });
 }
 int bscb200_coder_compress_device(void *ctx, const unsigned char *d_in, unsigned char *d_out, int n, int coder, int features)
 {
     Ctx *c = (Ctx *)ctx;
-    if (coder < 1 || coder > 3 || n <= 0) return LIBBSC_BAD_PARAMETER;
+    if (!coder_valid(coder) || n <= 0) return LIBBSC_BAD_PARAMETER;
     return guarded(c, [&]() { c->arena.reset(); c->arena.reserve(need_coder((size_t)n)); return stage_coder_compress(c, d_in, d_out, n, coder, features); });
 }
 int bscb200_coder_decompress_device(void *ctx, const unsigned char *d_in, int inputSize, unsigned char *d_out, int outputCapacity, int coder, int features)
 {
     Ctx *c = (Ctx *)ctx;
-    if (coder < 1 || coder > 3 || inputSize < 1 || outputCapacity < 0) return LIBBSC_BAD_PARAMETER;
+    if (!coder_valid(coder) || inputSize < 1 || outputCapacity < 0) return LIBBSC_BAD_PARAMETER;
     return guarded(c, [&]() { c->arena.reset(); c->arena.reserve(need_coder((size_t)outputCapacity)); return stage_coder_decompress(c, d_in, inputSize, d_out, outputCapacity, coder, features); });
 }
 unsigned int bscb200_adler32_device(void *ctx, const unsigned char *d_p, int n)

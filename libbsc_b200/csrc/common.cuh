@@ -114,8 +114,6 @@ struct Ctx {
     long long    sort_budget = 0;       // > 0: the forward BWT sorts in batches when its standard working set is larger (bscb200_ctx_set_sort_budget)
     u32         *h_mail = nullptr;      // pinned host mailbox (64 words) for small D2H read-backs
     u32         *d_mail = nullptr;      // device mailbox (64 words)
-    u8          *h_stage = nullptr;     // pinned staging for host<->device block copies
-    size_t       h_stage_cap = 0;
     u64          kernels_launched = 0;  // our own kernel launches enqueued through this ctx
     bool         profile = false;       // bracket every launch with CUDA events (bench.py roofline leg)
     double       next_bytes = 0;        // algorithmic bytes of the next launch (PROF_BYTES)
@@ -194,16 +192,6 @@ struct Ctx {
     void fetch_mail(int words) {
         CUDA_TRY(cudaMemcpyAsync(h_mail, d_mail, sizeof(u32) * words, cudaMemcpyDeviceToHost, stream));
         sync();
-    }
-    u8 *stage(size_t bytes) {
-        if (bytes > h_stage_cap) {
-            if (h_stage) cudaFreeHost(h_stage);
-            h_stage = nullptr; h_stage_cap = 0;
-            size_t want = align_up(bytes + (bytes >> 3) + 65536, 1 << 20);
-            CUDA_TRY(cudaMallocHost((void **)&h_stage, want));
-            h_stage_cap = want;
-        }
-        return h_stage;
     }
 };
 

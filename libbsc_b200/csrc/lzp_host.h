@@ -144,7 +144,9 @@ inline int encode_large(const unsigned char *in, const unsigned char *in_end, un
 //   word       4 or 8 bytes (T)
 //   second_at  offset of the second word that must agree, or -1 (small)
 //   guard      bytes kept clear at the end of the chunk: word (small) or 2 * word (small2x, medium)
-inline int encode_short(const unsigned char *in, const unsigned char *in_end, unsigned char *out, unsigned char *out_end, int *seen, uint32_t mask,
+// Always inlined, so that each of encode_chunk's five calls is its own copy with these as constants.  Left to the compiler, the choice
+// follows how much else api.cu inlines, and an out-of-line copy becomes one more symbol the library exports.
+inline __attribute__((always_inline)) int encode_short(const unsigned char *in, const unsigned char *in_end, unsigned char *out, unsigned char *out_end, int *seen, uint32_t mask,
                         int min_len, int word, int second_at, int guard)
 {
     const unsigned char *in_start = in, *out_start = out, *eob = out_end - 8;
