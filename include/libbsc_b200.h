@@ -58,8 +58,8 @@ int bsc_init_full(int features, void *(*malloc_fn)(size_t), void *(*zero_malloc_
  * n > 1 GiB is LIBBSC_BAD_PARAMETER as in the reference.  An in-place block above 1 GiB is sorted in place with the batched forward
  * BWT on a context of its own, in at most bscb200_inplace_bytes() = 18 n + 256 MiB of HBM, all of it freed when the call returns;
  * LIBBSC_GPU_NOT_ENOUGH_MEMORY (nothing written) when the device has less free.  The caller's buffer is written only on success.
- * Above 1 GiB bsc_compress with the sort transforms (blockSorter 3..8) returns LIBBSC_NOT_SUPPORTED: the forward ST needs about 30 n
- * and has no bounded variant.  bsc_decompress reads every block the reference writes, up to 2146435072 bytes with every sorter: a block
+ * Above 1 GiB bsc_compress with the sort transforms (blockSorter 3..8) returns LIBBSC_NOT_SUPPORTED; bsc_st_encode itself takes such
+ * blocks (below), so libbsc's own bsc_compress linked against this library's stages writes them.  bsc_decompress reads every block the reference writes, up to 2146435072 bytes with every sorter: a block
  * above 1 GiB runs on a context of its own, in at most bscb200_decompress_bytes() of HBM (18 n + 256 MiB for the BWT, 26.5 n + 256 MiB
  * for ST3..ST8), all of it freed when the call returns; LIBBSC_GPU_NOT_ENOUGH_MEMORY when the device has less free. */
 int bsc_compress(const unsigned char *input, unsigned char *output, int n, int lzpHashSize, int lzpMinLen, int blockSorter, int coder, int features);
@@ -77,6 +77,8 @@ int bsc_bwt_decode(unsigned char *T, int n, int index, unsigned char num_indexes
 
 /* libbsc/st/st.h:47,57,68 ; libbsc/st/st.cpp:990-1012 (k = 3..8; st.cu:334 for 7, 8).  In place on T. */
 int bsc_st_init(int features);
+/* bsc_st_encode above 1 GiB sorts in batches on a context of its own, in at most bscb200_st_encode_bytes(n) = 6 n + 256 MiB of HBM, all of
+ * it freed when the call returns; LIBBSC_GPU_NOT_ENOUGH_MEMORY (T untouched) when the device has less free.  T is written only on success. */
 int bsc_st_encode(unsigned char *T, int n, int k, int features);
 int bsc_st_decode(unsigned char *T, int n, int k, int index, int features);   /* st.h:68 ; st.cpp:1491-1527 (csrc/st_decode.cu) */
 
@@ -115,11 +117,13 @@ int bscb200_coder_decompress(const unsigned char *input, int inputSize, unsigned
 void              *bscb200_ctx_create(int device, void *cuda_stream);
 void               bscb200_ctx_destroy(void *ctx);
 int                bscb200_ctx_reserve(void *ctx, long long bytes);
-/* Bounds the forward BWT's working set on this context: whenever the standard sorter would need more than `bytes` (about 58 n + 64 MB
- * for a block of n), the sort runs in batches of B = (bytes - 16 n) / 32 entries in about 16 n + 32 B bytes.  Same results either way.
- * B is at least max(65536, n / 64): every key range of the initial sort and of an oversized group rescans its segment, so the work
- * grows with n / B, and the floor keeps it within about 64 passes over the block per such segment.  Smaller batches cost time: see
- * DESIGN.md 4.2 for measured times.  0 (the default) = no bound; negative = LIBBSC_BAD_PARAMETER.  Block sorters 3..8 ignore it.
+/* Bounds the working set of the forward sorts on this context.  BWT: whenever the standard sorter would need more than `bytes` (about
+ * 58 n + 64 MB for a block of n), the sort runs in batches of B = (bytes - 16 n) / 32 entries in about 16 n + 32 B bytes.  Sort
+ * transforms (block sorters 3..8, bscb200_st_encode_device and bscb200_compress_device): whenever the standard sorter would need more
+ * than `bytes` (30 n + 16 MB), in batches of B = (bytes - n) / 28 entries in about n + 28 B bytes.  Same results either way.
+ * B is at least max(65536, n / 64): every key range rescans the text (or an oversized group of the BWT), so the work grows with n / B,
+ * and the floor keeps it within about 64 passes over the block per such segment.  Smaller batches cost time: see DESIGN.md 4.2 and 4.3
+ * for measured times.  0 (the default) = no bound; negative = LIBBSC_BAD_PARAMETER.
  * bscb200_compress_device keeps its 1 GiB limit; blocks above it go through the in-place bsc_compress. */
 int                bscb200_ctx_set_sort_budget(void *ctx, long long bytes);
 int                bscb200_lzp_decompress_host(const unsigned char *input, int n, unsigned char *output, int outputCapacity, int lzpHashSize, int lzpMinLen);   /* inverse of the reference LZP stage (libbsc/lzp/lzp.h), host only */
@@ -139,6 +143,9 @@ long long          bscb200_inplace_bytes(int n, int blockSorter, int coder);
  * (= bscb200_inplace_bytes(n, 1, 1)) and 26.5 n + 256 MiB for ST3..ST8 (about 57.2 GB at n = 2146435072), none of it kept after the call.
  * Up to 1 GiB: the pooled cost, bscb200_workspace_bytes + bscb200_scratch_bytes.  Bad arguments: LIBBSC_BAD_PARAMETER. */
 long long          bscb200_decompress_bytes(int n, int blockSorter);
+/* HBM that bsc_st_encode of n bytes takes at most: above 1 GiB 6 n + 256 MiB (about 13.1 GB at n = 2146435072), none of it kept after
+ * the call; up to 1 GiB the pooled cost, the staged block (n + 4096) and one sort slab (30 n + 16 MiB).  Bad arguments: LIBBSC_BAD_PARAMETER. */
+long long          bscb200_st_encode_bytes(int n);
 unsigned long long bscb200_ctx_kernel_launches(void *ctx);
 unsigned long long bscb200_total_kernel_launches(void);
 /* per-kernel CUDA-event timing of everything launched through ctx (bench.py's roofline leg) */

@@ -66,6 +66,7 @@ _SIGNATURES = {
     "bscb200_scratch_bytes": ([ci, ci], ctypes.c_longlong),
     "bscb200_inplace_bytes": ([ci, ci, ci], ctypes.c_longlong),
     "bscb200_decompress_bytes": ([ci, ci], ctypes.c_longlong),
+    "bscb200_st_encode_bytes": ([ci], ctypes.c_longlong),
     "bscb200_ctx_kernel_launches": ([vp], ctypes.c_ulonglong),
     "bscb200_total_kernel_launches": ([], ctypes.c_ulonglong),
     "bscb200_ctx_set_profile": ([vp, ci], None),

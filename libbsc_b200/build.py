@@ -9,7 +9,7 @@ CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libbsc_b200.so")
 CLI = os.path.join(HERE, "bsc_b200")          # file-level front end (cli/bsc_b200.cpp), bsc1 container + multi-GPU block scheduler
-SOURCES = ["api.cu", "adler32.cu", "bwt_encode.cu", "bwt_encode_batched.cu", "bwt_decode.cu", "st_encode.cu", "st_decode.cu", "qlfc.cu"]
+SOURCES = ["api.cu", "adler32.cu", "bwt_encode.cu", "bwt_encode_batched.cu", "bwt_decode.cu", "st_encode.cu", "st_encode_batched.cu", "st_decode.cu", "qlfc.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
          "-Xcompiler", "-fPIC,-O2,-Wall,-Wno-unused-function", "-ccbin", "/usr/bin/g++",

@@ -331,6 +331,18 @@ int bwt_encode_leased(Ctx *ctx, u8 *d_T, int n, unsigned char *num_indexes, int 
     return stage_bwt_encode_batched(ctx, d_T, n, num_indexes, indexes, B);
 }
 
+// The same for the forward sort transform of order k (block sorters 3..8)
+int st_encode_leased(Ctx *ctx, u8 *d_T, int n, int k)
+{
+    if (ctx->sort_budget <= 0 || n <= 1 || (long long)need_st_encode((size_t)n) <= ctx->sort_budget) {
+        ScratchLease lease(ctx, need_st_encode((size_t)n));
+        return stage_st_encode(ctx, d_T, n, k);
+    }
+    const u32 B = st_batch_entries((u32)n, ctx->sort_budget);
+    ScratchLease lease(ctx, st_batched_bytes((u32)n, B));
+    return stage_st_encode_batched(ctx, d_T, n, k, B);
+}
+
 // ---------------------------------------------------------------------------------------------
 // block compress
 // ---------------------------------------------------------------------------------------------
@@ -409,7 +421,7 @@ int compress_dev(Ctx *ctx, const u8 *d_in, int n, u8 *d_out, int blockSorter, in
 
     int indexes[256]; unsigned char num_indexes = 0;
     if (blockSorter == 1) H.index = bwt_encode_leased(ctx, work, n, &num_indexes, indexes);      // the sort's ~58 n live in a shared slab
-    else { ScratchLease lease(ctx, need_st_encode(n)); H.index = stage_st_encode(ctx, work, n, blockSorter); }
+    else H.index = st_encode_leased(ctx, work, n, blockSorter);
     if (H.data_size < 64 * 1024) num_indexes = 0;       // libbsc.cpp:303
     if (H.index < 0) { A.release(mark); return H.index; }
 
@@ -519,8 +531,8 @@ int decompress_dev(Ctx *ctx, const BlockHeader &H, const u8 *d_block, u8 *d_out,
 // the context, and a 16.5 n sort slab that the pool keeps after the call.  A block above 1 GiB instead runs on a context made for the
 // call and destroyed after it, in ONE allocation: the block, sorted in place (an in-place call may destroy its input, libbsc.cpp:160),
 // and a region that first holds the batched forward BWT (16 n + 32 B) and then the coder stage with its output (about 9.5 n + 28 MB).
-// The caller's buffer is written only once the block is done.  Only the BWT has a bounded forward sorter: the forward ST needs about
-// 30 n (need_st_encode), so ST3..ST8 compress only up to 1 GiB.  Their inverse has a lean layout (decompress_large_st below).
+// The caller's buffer is written only once the block is done.  In place, ST3..ST8 compress only up to 1 GiB; bsc_st_encode above it has
+// a bounded path of its own (st_encode_large below), and their inverse a lean layout (decompress_large_st below).
 // The arena is 17.5 n + 128 MiB: the batched sort at batches of about n / 64 entries (16.5 n) or the coder stage with its output
 // (at most 9.5 n + 28 MB) after the block.  The bound adds n / 2 + 128 MiB for what lies outside the arena: the context, the coder
 // tables, kernel images loaded on first use and the driver's own transient allocations (about 0.55 GB measured at the largest n).
@@ -551,6 +563,11 @@ size_t large_arena(size_t n) { return 17 * n + n / 2 + LARGE_FIXED / 2; }
 size_t large_st_region(size_t n) { return std::max(st_decode_lean_bytes(n), align_up(n + 28 + 128, 256) + need_coder(n)); }
 size_t large_st_arena(size_t n) { return align_up(n + 128 + 256, 256) + align_up(large_st_region(n), 256); }
 size_t large_st_bound(size_t n) { return 26 * n + n / 2 + LARGE_FIXED; }
+// bsc_st_encode of a block above 1 GiB: ONE arena of 5.5 n + 128 MiB holds the staged block (n + 64) and the batched forward ST after it
+// (st_batched_bytes: L, n bytes, and 28 bytes per batch entry), whose batches take what is left: about n / 8 entries.  The bound adds
+// n / 2 + 128 MiB for what lies outside the arena, as large_bound does: 6 n + 256 MiB, 13.1 GB at n = 2146435072.
+size_t st_large_arena(size_t n) { return 5 * n + n / 2 + LARGE_FIXED / 2; }
+size_t st_large_bound(size_t n) { return 6 * n + LARGE_FIXED; }
 
 // In-place bsc_compress of a block of n > 1 GiB bytes with the BWT sorter (libbsc.cpp:124-210).
 int compress_large(unsigned char *data, int n, int lzpHashSize, int lzpMinLen, int coder, int features)
@@ -613,6 +630,26 @@ int decompress_large_st(const unsigned char *input, const BlockHeader &H, unsign
         const int r = stage_st_decode_lean(ctx, d_L, lzSize, H.mode.sorter(), H.index, &d_T);
         if (r < 0) return r;
         return deliver(ctx, H, d_T, lzSize, output);
+    });
+}
+
+// bsc_st_encode of T (n bytes) above the routing threshold (st_large_arena above).  The caller checked the arguments.  T is written only
+// on success.
+int st_encode_large(unsigned char *T, int n, int k)
+{
+    size_t fr = 0, total = 0;
+    if (cudaMemGetInfo(&fr, &total) != cudaSuccess) { cudaGetLastError(); return LIBBSC_GPU_NOT_SUPPORTED; }
+    if (fr < st_large_bound((size_t)n)) return LIBBSC_GPU_NOT_ENOUGH_MEMORY;
+    return with_own_ctx([&](Ctx *ctx) {
+        Arena &A = ctx->arena;
+        A.reserve(st_large_arena((size_t)n));
+        u8 *d = A.get<u8>((size_t)n + 64);
+        CUDA_TRY(cudaMemcpyAsync(d, T, (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
+        // the sort may use the rest of the arena (less a margin for its rounding)
+        const u32 B = st_batch_entries((u32)n, (long long)(A.cap - A.used) - (16ll << 20));
+        const int r = stage_st_encode_batched(ctx, d, n, k, B);
+        if (r >= 0) { CUDA_TRY(cudaMemcpyAsync(T, d, (size_t)n, cudaMemcpyDeviceToHost, ctx->stream)); ctx->sync(); }
+        return r;
     });
 }
 
@@ -791,7 +828,8 @@ int bsc_st_encode(unsigned char *T, int n, int k, int features)
     if (T == nullptr || n < 0) return LIBBSC_BAD_PARAMETER;
     if (!st_order_valid(k)) return LIBBSC_BAD_PARAMETER;
     if (n <= 1) return 0;
-    return stage_in_place(T, n, (size_t)n + 4096, [&](Ctx *ctx, u8 *d) { ScratchLease lease(ctx, need_st_encode(n)); return stage_st_encode(ctx, d, n, k); });
+    if (n > large_route_n()) return st_encode_large(T, n, k);
+    return stage_in_place(T, n, (size_t)n + 4096, [&](Ctx *ctx, u8 *d) { return st_encode_leased(ctx, d, n, k); });
 }
 
 int bsc_st_decode(unsigned char *T, int n, int k, int index, int features)
@@ -896,8 +934,8 @@ int bscb200_ctx_reserve(void *ctx, long long bytes)
     Ctx *c = (Ctx *)ctx;
     return guarded(c, [&]() { CUDA_TRY(cudaSetDevice(c->device)); c->arena.reset(); c->arena.reserve((size_t)bytes); return 0; });
 }
-// Bounds the forward BWT's working set on this context: it sorts in batches whenever the standard sorter would need more than `bytes`
-// (0 = no bound).  Block sorters 3..8 ignore it.
+// Bounds the working set of the forward sorts on this context, the BWT and the sort transforms (block sorters 3..8): each sorts in
+// batches whenever its standard sorter would need more than `bytes` (0 = no bound).
 int bscb200_ctx_set_sort_budget(void *ctx, long long bytes)
 {
     if (!ctx || bytes < 0) return LIBBSC_BAD_PARAMETER;
@@ -921,8 +959,16 @@ long long bscb200_scratch_bytes(int n, int blockSorter)     /* size of one share
 long long bscb200_inplace_bytes(int n, int blockSorter, int coder)
 {
     if (n < 0 || n > 2146435072 || !sorter_valid(blockSorter) || !coder_valid(coder)) return LIBBSC_BAD_PARAMETER;
-    if (blockSorter != 1) return LIBBSC_NOT_SUPPORTED;      // no bounded sort transform
+    if (blockSorter != 1) return LIBBSC_NOT_SUPPORTED;      // the in-place bsc_compress does not encode ST3..ST8 above 1 GiB
     return (long long)large_bound((size_t)n);
+}
+// HBM that bsc_st_encode of n bytes takes at most: above 1 GiB the bound of its own context (st_large_bound), else the pooled cost, the
+// staged block in a context and one shared sort slab
+long long bscb200_st_encode_bytes(int n)
+{
+    if (n < 0 || n > 2146435072) return LIBBSC_BAD_PARAMETER;
+    if (n > LARGE_N) return (long long)st_large_bound((size_t)n);
+    return (long long)((size_t)n + 4096 + need_st_encode((size_t)n));
 }
 // HBM that bsc_decompress of a block with data size n takes at most: above 1 GiB the bound of its own context (large_bound for the BWT,
 // large_st_bound for ST3..ST8), else the pooled cost, one context's workspace and one shared sort slab
@@ -1009,7 +1055,7 @@ int bscb200_st_encode_device(void *ctx, unsigned char *d_T, int n, int k)
 {
     Ctx *c = (Ctx *)ctx;
     if (d_T == nullptr || n < 0 || !st_order_valid(k)) return LIBBSC_BAD_PARAMETER;
-    return guarded(c, [&]() { c->arena.reset(); ScratchLease lease(c, need_st_encode((size_t)n)); return stage_st_encode(c, d_T, n, k); });
+    return guarded(c, [&]() { c->arena.reset(); return st_encode_leased(c, d_T, n, k); });
 }
 int bscb200_st_decode_device(void *ctx, unsigned char *d_T, int n, int k, int index)
 {

@@ -19,6 +19,14 @@ int stage_bwt_decode(Ctx *ctx, u8 *d_T, int n, int index);
 size_t bwt_decode_bytes(u32 n);
 // Sort transform of order k in place (bsc_st_encode, st.cpp:990; k = 3..8).
 int stage_st_encode(Ctx *ctx, u8 *d_T, int n, int k);
+// The same result with a bounded working set (st_encode_batched.cu): sorts in batches of at most B entries (raised to bwt_batch_floor(n)
+// if smaller) and takes st_batched_bytes(n, B) from ctx->sort_arena(); d_T needs no padding or alignment and is written only at the end.
+int stage_st_encode_batched(Ctx *ctx, u8 *d_T, int n, int k, u32 B);
+size_t st_batched_bytes(u32 n, u32 B);
+// batch entries that a working set of `budget` bytes allows at block length n (at least bwt_batch_floor(n), at most that, n or
+// ST_BATCH_MAX, which keeps every radix sort far below the 2^30 entries rs_onesweep assumes whatever the block length)
+#define ST_BATCH_MAX (1 << 28)
+u32 st_batch_entries(u32 n, long long budget);
 // Inverse sort transform in place (bsc_st_decode, st.cpp:1491; k = 3..8, index = row of rotation 0).
 int stage_st_decode(Ctx *ctx, u8 *d_T, int n, int k, int index);
 // The same inverse in the lean layout of the blocks above 1 GiB (st_decode.cu): L is read at d_L, which needs n + 64 writable bytes, and
