@@ -16,7 +16,20 @@
 //      re-split groups, scatter the new ranks, compact away the newly unique suffixes.
 //   4. Emit L, the primary index and the secondary indexes straight from rank[].
 //
-// All intermediate arrays live in the Ctx arena (about 53 n bytes).
+// Segmented rounds (BSCB200_BWT_SEG = S, default 256; 0 = off).  Each group already occupies a contiguous range of the round's
+// slots and only needs ordering by key2 inside it, so step 3's global sort over (group, key2) can be split by group size:
+//   - groups of at most S entries are sorted inside one CTA (bwt_seg_sort): a CTA owns the groups that START in its
+//     SEG_TILE slots, loads them whole (at most SEG_TILE - 1 + S <= SEG_CAP entries) into shared memory, places each
+//     entry by counting the smaller key2 of its group and writes it to its slot -- one read and one write instead of up to 8
+//     radix passes;
+//   - the larger groups are compacted (bwt_seg_compact), radix-sorted by (dense large-group id, key2) -- fewer group bits
+//     than the dense id over all groups -- and written back to their slot ranges (bwt_seg_scatter).
+// The result is the array the global sort gives, up to the order of equal (group, key2) entries, which the split does not
+// see: it gives them one rank.  So L and the indexes are unchanged.  The group starts live in idx[ib ^ 1] (free until
+// bwt_apply writes it) and the large entries in k[] / v[], so the arena is the same size.
+// On a 64 MiB text block S = 256 takes the forward BWT from 37.4 to 35.4 ms (DESIGN 4.2): larger S spend more on counting
+// inside large groups than they save in radix passes, smaller ones leave more entries to the radix sort.
+//
 #include "radix_sort.cuh"
 #include "stages.cuh"
 #include "bwt_rounds.cuh"
@@ -36,6 +49,115 @@ struct SrcRound {
     __device__ __forceinline__ u64 key(u32 e) const { return ((u64)grp[e] << 32) | key2[e]; }
     __device__ __forceinline__ u32 val(u32 e) const { return sa[e]; }
 };
+
+#define SEG_TILE    1024                              // slots whose groups one bwt_seg_sort CTA owns
+#define SEG_CAP     2048                              // entries it can hold: SEG_TILE - 1 + S for the largest S
+#define SEG_MAX     (SEG_CAP - SEG_TILE)
+#define SEG_DEFAULT 256                               // measured best of 64 / 256 / 1024 on a 64 MiB text block (DESIGN 4.2)
+
+// the group-size bound of the segmented rounds (0: every group goes through the global radix sort), read once per process
+static u32 bwt_seg_limit()
+{
+    static const u32 v = [] { const char *e = getenv("BSCB200_BWT_SEG"); const int k = e ? atoi(e) : SEG_DEFAULT; return (u32)(k < 0 ? 0 : k > SEG_MAX ? SEG_MAX : k); }();
+    return v;
+}
+
+// gstart[g] = first slot of group g, gstart[G] = m (grp[] is dense and ascending in slot order)
+__global__ void __launch_bounds__(256) bwt_seg_starts(const u32 *__restrict__ grp, u32 *__restrict__ gstart, u32 m, u32 G)
+{
+    const u32 t = blockIdx.x * 256 + threadIdx.x;
+    if (t >= m) return;
+    const u32 g = grp[t];
+    if (t == 0 || grp[t - 1] != g) gstart[g] = t;
+    if (t == 0) gstart[G] = m;
+}
+
+// The entries of groups of more than S entries, per SC_TILE slots (warp w takes slots w*256 + 32 i + lane, which keeps slot order).
+//   SEG_COUNT:   tile totals of large entries and large groups -> agg (then bwt_tile_scan makes them exclusive prefixes)
+//   SEG_COMPACT: large entry number e <- ((dense large-group id) << 32 | key2, sa)
+//   SEG_SCATTER: slot t <- (grp << 32 | key2 of sorted entry e, its sa)
+enum { SEG_COUNT, SEG_COMPACT, SEG_SCATTER };
+template <int MODE>
+__global__ void __launch_bounds__(SC_THREADS) bwt_seg_large(const u32 *__restrict__ grp, const u32 *__restrict__ key2, const u32 *__restrict__ sa,
+                                                            const u32 *__restrict__ gstart, u32 m, u32 S, TileAgg *__restrict__ agg,
+                                                            const u64 *__restrict__ kin, const u32 *__restrict__ vin, u64 *__restrict__ kout, u32 *__restrict__ vout)
+{
+    __shared__ u32 s_cnt[SC_THREADS / 32], s_hd[SC_THREADS / 32];
+    const u32 lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    const u32 base = blockIdx.x * SC_TILE + w * (32 * SC_ITEMS) + lane;
+    u32 g[SC_ITEMS], big[SC_ITEMS], head[SC_ITEMS], cnt = 0, hds = 0;
+#pragma unroll
+    for (int i = 0; i < SC_ITEMS; ++i) {
+        const u32 t = base + 32 * i;
+        bool L = false, H = false;
+        g[i] = 0;
+        if (t < m) { g[i] = grp[t]; const u32 s0 = gstart[g[i]]; L = gstart[g[i] + 1] - s0 > S; H = s0 == t; }
+        big[i] = __ballot_sync(0xffffffffu, L); head[i] = __ballot_sync(0xffffffffu, L && H);
+        cnt += __popc(big[i]); hds += __popc(head[i]);
+    }
+    if (lane == 0) { s_cnt[w] = cnt; s_hd[w] = hds; }
+    __syncthreads();
+    if (MODE == SEG_COUNT) {
+        if (threadIdx.x == 0) {
+            for (int i = 1; i < SC_THREADS / 32; ++i) { cnt += s_cnt[i]; hds += s_hd[i]; }
+            agg[blockIdx.x] = TileAgg{0, cnt, hds, 0};
+        }
+        return;
+    }
+    const TileAgg carry = agg[blockIdx.x];
+    u32 e = carry.active, lid = carry.groups;
+    for (u32 i = 0; i < w; ++i) { e += s_cnt[i]; lid += s_hd[i]; }
+    const u32 lt = lanemask_lt(), le = lt | (1u << lane);
+#pragma unroll
+    for (int i = 0; i < SC_ITEMS; ++i) {
+        const u32 t = base + 32 * i;
+        if ((big[i] >> lane) & 1u) {
+            const u32 my = e + __popc(big[i] & lt);
+            if (MODE == SEG_COMPACT) { kout[my] = ((u64)(lid + __popc(head[i] & le) - 1) << 32) | key2[t]; vout[my] = sa[t]; }
+            else                     { kout[t] = ((u64)g[i] << 32) | (u32)kin[my]; vout[t] = vin[my]; }
+        }
+        e += __popc(big[i]); lid += __popc(head[i]);
+    }
+}
+
+// The groups of at most S entries that start in slots [blockIdx.x * SEG_TILE, + SEG_TILE): loaded whole (a group of more than S
+// entries at the end is left out; one in the middle is loaded but skipped) into shared memory.  Each entry's place in its group is
+// the number of entries of the group with a smaller key2, or an equal one at a smaller slot: a count over the group, which the warp
+// reads as broadcasts.  That costs s steps per entry of a group of s, far fewer than a sorting network over the CTA's 2048 entries
+// for the small groups that hold most entries.  16 KB of shared memory, so a CTA fits next to the coder CTAs of the pipeline.
+__global__ void __launch_bounds__(256) bwt_seg_sort(const u32 *__restrict__ grp, const u32 *__restrict__ key2, const u32 *__restrict__ sa,
+                                                    const u32 *__restrict__ gstart, u32 m, u32 S, u64 *__restrict__ kout, u32 *__restrict__ vout)
+{
+    __shared__ u32 sk[SEG_CAP];
+    __shared__ u32 sv[SEG_CAP];
+    __shared__ u32 s_a, s_b;
+    const u32 tid = threadIdx.x, base = blockIdx.x * SEG_TILE, end = min(base + SEG_TILE, m);
+    if (tid == 0) {
+        const u32 g0 = grp[base];
+        const u32 a = gstart[g0] == base ? base : gstart[g0 + 1];
+        u32 b = a;
+        if (a < end) {
+            const u32 g1 = grp[end - 1], s1 = gstart[g1];
+            b = gstart[g1 + 1];
+            if (b - s1 > S) b = s1;
+        }
+        s_a = a; s_b = max(a, b);
+    }
+    __syncthreads();
+    const u32 a = s_a, len = s_b - a;
+    if (len == 0) return;
+    for (u32 j = tid; j < len; j += 256) { sk[j] = key2[a + j]; sv[j] = sa[a + j]; }
+    __syncthreads();
+    for (u32 j = tid; j < len; j += 256) {
+        const u32 g = grp[a + j], gs = gstart[g], ge = gstart[g + 1];
+        if (ge - gs > S) continue;
+        const u32 my = sk[j], lo = gs - a, hi = ge - a;
+        u32 pos = 0;
+        for (u32 i = lo; i < hi; ++i) { const u32 x = sk[i]; pos += (x < my) | ((x == my) & (i < j)); }
+        kout[gs + pos] = ((u64)g << 32) | my;
+        vout[gs + pos] = sv[j];
+    }
+}
 
 }  // namespace
 
@@ -87,11 +209,34 @@ int stage_bwt_encode(Ctx *ctx, u8 *d_T, int n_, unsigned char *num_indexes, int 
 
     // 3. doubling rounds
     const int bits_k2 = bits_for(n);
+    const u32 S = bwt_seg_limit();
     for (u64 h = 8; m > 0; h <<= 1) {
         if (h >= ((u64)1 << 31)) { A.release(mark); return LIBBSC_GPU_ERROR; }   // cannot happen for n < 2^31: no group survives h >= n, so the last round needed is h = 2^30
         LAUNCH(ctx, bwt_gather_key2, ceil_div(m, 256), 256, 0, sa_act, rank, key2, m, n, (u32)h);
-        DigitPasses pr = make_passes(0, bits_k2, 32, 32 + (G > 1 ? bits_for(G - 1) : 0));
-        cur = rs_sort<u64, true>(ctx, SrcRound{grp, key2, sa_act}, k, v, m, pr, scratch);
+        if (S == 0) {
+            DigitPasses pr = make_passes(0, bits_k2, 32, 32 + (G > 1 ? bits_for(G - 1) : 0));
+            cur = rs_sort<u64, true>(ctx, SrcRound{grp, key2, sa_act}, k, v, m, pr, scratch);
+        } else {
+            u32 *gstart = idx[ib ^ 1];                   // G + 1 <= m / 2 + 1 words; bwt_apply writes idx[ib ^ 1] only after the sort
+            LAUNCH(ctx, bwt_seg_starts, ceil_div(m, 256), 256, 0, grp, gstart, m, G);
+            tiles = ceil_div(m, SC_TILE);
+            LAUNCH_NAMED(ctx, "bwt_seg_count", bwt_seg_large<SEG_COUNT>, tiles, SC_THREADS, 0, grp, key2, sa_act, gstart, m, S, agg,
+                         (const u64 *)nullptr, (const u32 *)nullptr, (u64 *)nullptr, (u32 *)nullptr);
+            LAUNCH(ctx, bwt_tile_scan, 1, 1024, 0, agg, tiles, ctx->d_mail);
+            ctx->fetch_mail(2);
+            const u32 ml = ctx->h_mail[0], nl = ctx->h_mail[1];   // entries and number of the groups of more than S entries
+            cur = 0;
+            if (ml > 0) {
+                LAUNCH_NAMED(ctx, "bwt_seg_compact", bwt_seg_large<SEG_COMPACT>, tiles, SC_THREADS, 0, grp, key2, sa_act, gstart, m, S, agg,
+                             (const u64 *)nullptr, (const u32 *)nullptr, k[1], v[1]);
+                DigitPasses pl = make_passes(0, bits_k2, 32, 32 + (nl > 1 ? bits_for(nl - 1) : 0));
+                const int c = rs_sort<u64, true>(ctx, SrcArray<u64, true>{k[1], v[1]}, k, v, ml, pl, scratch);   // pass 0 reads k[1] before pass 1 writes it
+                cur = c ^ 1;
+                LAUNCH_NAMED(ctx, "bwt_seg_scatter", bwt_seg_large<SEG_SCATTER>, tiles, SC_THREADS, 0, grp, key2, sa_act, gstart, m, S, agg,
+                             (const u64 *)k[c], (const u32 *)v[c], k[cur], v[cur]);
+            }
+            if (ml < m) LAUNCH(ctx, bwt_seg_sort, ceil_div(m, SEG_TILE), 256, 0, grp, key2, sa_act, gstart, m, S, k[cur], v[cur]);
+        }
         tiles = ceil_div(m, SC_TILE);
         LAUNCH(ctx, bwt_tile_reduce<false>, tiles, SC_THREADS, 0, k[cur], v[cur], idx[ib], m, n, agg);
         LAUNCH(ctx, bwt_tile_scan, 1, 1024, 0, agg, tiles, ctx->d_mail);
