@@ -30,6 +30,14 @@
 // On a 64 MiB text block S = 256 takes the forward BWT from 37.4 to 35.4 ms (DESIGN 4.2): larger S spend more on counting
 // inside large groups than they save in radix passes, smaller ones leave more entries to the radix sort.
 //
+// Staged rank and L stores (BSCB200_BWT_STAGE: 0 = direct, 1 = staged, unset = by size, stage_on).  rank[sa] = value in bwt_apply
+// and L[row] = byte in bwt_emit are random stores into arrays larger than the L2; each one leaves a sector partly written.  Staged,
+// the kernels write (value << 32 | position) pairs in slot order instead, one keys-only radix pass partitions them by the top 8
+// position bits, and bwt_stage_scatter stores them in that order: the resident CTAs then write into a few windows at a time, whose
+// sectors the L2 merges whole.  The pairs of a split go to k[cur ^ 1] (idle during bwt_apply) and are partitioned into k[cur] (dead
+// once bwt_apply has read it); those of the emit use k[1] and k[0].  So the arena is unchanged.  A 64 MiB text block, every store
+// staged: 36.4 -> 28.8 ms.
+//
 #include "radix_sort.cuh"
 #include "stages.cuh"
 #include "bwt_rounds.cuh"
@@ -159,6 +167,49 @@ __global__ void __launch_bounds__(256) bwt_seg_sort(const u32 *__restrict__ grp,
     }
 }
 
+// dst[pos] = value for the pairs (value << 32 | pos), read in order: after the partition by window, the stores of the resident CTAs
+// fall into a few windows, whose sectors the L2 fills completely before it writes them back
+template <typename T>
+__global__ void __launch_bounds__(256) bwt_stage_scatter(const u64 *__restrict__ pairs, T *__restrict__ dst, u32 cnt)
+{
+    const u32 t = blockIdx.x * 256 + threadIdx.x;
+    if (t >= cnt) return;
+    const u64 p = pairs[t];
+    dst[(u32)p] = (T)(p >> 32);
+}
+
+// Staged scatter: the pairs (value << 32 | pos) in pairs[0..cnt), with every pos < 2^pos_bits, are partitioned by the top 8 bits of
+// pos (one keys-only radix pass, stable, into `parted`), then stored window after window.  The stores land where the direct
+// scatter puts them; only their order changes.
+template <typename T>
+static void bwt_stage_store(Ctx *ctx, const char *name, const u64 *pairs, u64 *parted, u32 cnt, int pos_bits, T *dst, void *scratch)
+{
+    u64 *const kk[2] = { parted, parted };              // one pass: it writes kk[0] only
+    u32 *const vv[2] = { nullptr, nullptr };
+    rs_sort<u64, false>(ctx, SrcArray<u64, false>{pairs, nullptr}, kk, vv, cnt, make_passes(pos_bits > 8 ? pos_bits - 8 : 0, pos_bits), scratch,
+                        "bwt_stage_part");
+    LAUNCH_NAMED(ctx, name, bwt_stage_scatter<T>, ceil_div(cnt, 256), 256, 0, parted, dst, cnt);
+}
+
+// Measured on an H100 (DESIGN 4.2): staged wins for 7.9 M entries and up, loses at 0.45 M; it loses on an L of 25 MiB (which the
+// 50 MB L2 holds) and wins on one of 64 MiB and on rank arrays of 100 and 256 MiB.
+#define STAGE_MIN_ENTRIES (1u << 22)
+#define STAGE_MIN_BYTES   ((size_t)50000000)
+
+// BSCB200_BWT_STAGE: 0 = every rank and L store direct, 1 = every one staged, unset = by size (stage_on); read once per process
+static int bwt_stage_switch()
+{
+    static const int v = [] { const char *e = getenv("BSCB200_BWT_STAGE"); return e && (e[0] == '0' || e[0] == '1') ? e[0] - '0' : -1; }();
+    return v;
+}
+
+// staged or direct store of cnt entries into an array of `bytes`
+static bool stage_on(u32 cnt, size_t bytes)
+{
+    const int s = bwt_stage_switch();
+    return s >= 0 ? s == 1 : (cnt >= STAGE_MIN_ENTRIES && bytes > STAGE_MIN_BYTES);
+}
+
 }  // namespace
 
 // Forward BWT of d_T[0..n) (device, in place).  Returns the primary index (>= 1) or an error.
@@ -203,7 +254,15 @@ int stage_bwt_encode(Ctx *ctx, u8 *d_T, int n_, unsigned char *num_indexes, int 
     LAUNCH(ctx, bwt_tile_reduce<true>, tiles, SC_THREADS, 0, k[cur], v[cur], (const u32 *)nullptr, m, n, agg);
     LAUNCH(ctx, bwt_tile_scan, 1, 1024, 0, agg, tiles, ctx->d_mail);
     int ib = 0;
-    LAUNCH(ctx, bwt_apply<true>, tiles, SC_THREADS, 0, k[cur], v[cur], (const u32 *)nullptr, m, n, agg, rank, sa_act, idx[ib], grp);
+    // the pairs of a staged rank store go to k[cur ^ 1], idle during bwt_apply, and are partitioned into k[cur], dead once it has run
+    const int pos_bits = bits_for(n - 1);
+    if (stage_on(m, (size_t)4 * n)) {
+        LAUNCH_NAMED(ctx, "bwt_apply_staged", (bwt_apply<true, false, true>), tiles, SC_THREADS, 0, k[cur], v[cur], (const u32 *)nullptr, m, n, agg,
+                     rank, sa_act, idx[ib], grp, k[cur ^ 1]);
+        bwt_stage_store(ctx, "bwt_stage_rank", k[cur ^ 1], k[cur], m, pos_bits, rank, scratch);
+    } else {
+        LAUNCH(ctx, bwt_apply<true>, tiles, SC_THREADS, 0, k[cur], v[cur], (const u32 *)nullptr, m, n, agg, rank, sa_act, idx[ib], grp);
+    }
     ctx->fetch_mail(2);
     m = ctx->h_mail[0]; u32 G = ctx->h_mail[1];
 
@@ -240,14 +299,25 @@ int stage_bwt_encode(Ctx *ctx, u8 *d_T, int n_, unsigned char *num_indexes, int 
         tiles = ceil_div(m, SC_TILE);
         LAUNCH(ctx, bwt_tile_reduce<false>, tiles, SC_THREADS, 0, k[cur], v[cur], idx[ib], m, n, agg);
         LAUNCH(ctx, bwt_tile_scan, 1, 1024, 0, agg, tiles, ctx->d_mail);
-        LAUNCH(ctx, bwt_apply<false>, tiles, SC_THREADS, 0, k[cur], v[cur], idx[ib], m, n, agg, rank, sa_act, idx[ib ^ 1], grp);
+        if (stage_on(m, (size_t)4 * n)) {
+            LAUNCH_NAMED(ctx, "bwt_apply_staged", (bwt_apply<false, true, true>), tiles, SC_THREADS, 0, k[cur], v[cur], idx[ib], m, n, agg,
+                         rank, sa_act, idx[ib ^ 1], grp, k[cur ^ 1]);
+            bwt_stage_store(ctx, "bwt_stage_rank", k[cur ^ 1], k[cur], m, pos_bits, rank, scratch);
+        } else {
+            LAUNCH(ctx, bwt_apply<false>, tiles, SC_THREADS, 0, k[cur], v[cur], idx[ib], m, n, agg, rank, sa_act, idx[ib ^ 1], grp);
+        }
         ib ^= 1;
         ctx->fetch_mail(2);
         m = ctx->h_mail[0]; G = ctx->h_mail[1];
     }
 
-    // 4. emit
-    LAUNCH(ctx, bwt_emit, ceil_div(n, 256), 256, 0, Tp, rank, d_T, n);
+    // 4. emit (every k / v buffer is free now)
+    if (stage_on(n - 1, n)) {
+        LAUNCH_NAMED(ctx, "bwt_emit_staged", bwt_emit<true>, ceil_div(n, 256), 256, 0, Tp, rank, d_T, n, k[1]);
+        bwt_stage_store(ctx, "bwt_stage_L", k[1], k[0], n - 1, pos_bits, d_T, scratch);
+    } else {
+        LAUNCH(ctx, bwt_emit, ceil_div(n, 256), 256, 0, Tp, rank, d_T, n);
+    }
     u32 cnt = want_aux ? (n - 1) / r : 0;
     LAUNCH(ctx, bwt_emit_indexes, 1, 256, 0, rank, n, r ? r : 1u, cnt, ctx->d_mail);
     ctx->fetch_mail(1 + (int)cnt);

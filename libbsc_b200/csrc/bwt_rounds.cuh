@@ -116,10 +116,13 @@ __global__ void __launch_bounds__(1024) bwt_tile_scan(TileAgg *agg, u32 tiles, u
     if (threadIdx.x == 1023) { mail[0] = pact + iact; mail[1] = pgrp + igrp; }
 }
 
-template <bool INIT, bool IDX = !INIT>
+// STAGE: instead of storing rank[sa] directly, write the pair (rank << 32 | sa) of slot t to rank_pairs[t], coalesced through the
+// tile's key array; bwt_encode.cu partitions the pairs by position window and stores them with bwt_stage_scatter.
+template <bool INIT, bool IDX = !INIT, bool STAGE = false>
 __global__ void __launch_bounds__(SC_THREADS) bwt_apply(const u64 *__restrict__ key, const u32 *__restrict__ sa, const u32 *__restrict__ idx,
                                                         u32 m, u32 n, const TileAgg *__restrict__ agg, u32 *__restrict__ rank,
-                                                        u32 *__restrict__ sa_out, u32 *__restrict__ idx_out, u32 *__restrict__ grp_out)
+                                                        u32 *__restrict__ sa_out, u32 *__restrict__ idx_out, u32 *__restrict__ grp_out,
+                                                        u64 *__restrict__ rank_pairs = nullptr)
 {
     __shared__ u32 s_max[SC_THREADS / 32], s_act[SC_THREADS / 32], s_grp[SC_THREADS / 32];
     __shared__ ScTile T;
@@ -156,21 +159,31 @@ __global__ void __launch_bounds__(SC_THREADS) bwt_apply(const u64 *__restrict__ 
         u32 t = base + i;
         if (t < m) {
             if (head[i]) { xmx = iv[i] + 1; if (!single[i]) xgrp++; }
-            rank[sv[i]] = xmx;                           // = 1 + SA slot of the group head
+            if (STAGE) T.key[sc_pad(threadIdx.x * SC_ITEMS + i)] = ((u64)xmx << 32) | sv[i];   // T.key was last read before the barrier above
+            else       rank[sv[i]] = xmx;                // = 1 + SA slot of the group head
             if (!single[i]) { sa_out[xact] = sv[i]; idx_out[xact] = iv[i]; grp_out[xact] = xgrp - 1; xact++; }
         }
+    }
+    if (STAGE) {
+        __syncthreads();
+        const u32 tbase = blockIdx.x * SC_TILE;
+        for (u32 j = threadIdx.x; j < SC_TILE && tbase + j < m; j += SC_THREADS) rank_pairs[tbase + j] = T.key[sc_pad(j)];
     }
 }
 
 // L, primary index and secondary indexes from the final ranks (Appendix B.1 of SURVEY.md)
-__global__ void __launch_bounds__(256) bwt_emit(const u8 *__restrict__ T, const u32 *__restrict__ rank, u8 *__restrict__ L, u32 n)
+// STAGE: row 0 is stored here; the other rows go as pairs (byte << 32 | row) to L_pairs[i - 1], for bwt_stage_scatter.
+template <bool STAGE = false>
+__global__ void __launch_bounds__(256) bwt_emit(const u8 *__restrict__ T, const u32 *__restrict__ rank, u8 *__restrict__ L, u32 n,
+                                                u64 *__restrict__ L_pairs = nullptr)
 {
     u32 i = blockIdx.x * 256 + threadIdx.x;
     if (i >= n) return;
     u32 p = __ldg(rank) - 1;                             // SA slot of suffix 0
     if (i == 0) { L[0] = T[n - 1]; return; }
     u32 j = rank[i] - 1;
-    L[j < p ? j + 1 : j] = T[i - 1];
+    if (STAGE) L_pairs[i - 1] = ((u64)T[i - 1] << 32) | (j < p ? j + 1 : j);
+    else       L[j < p ? j + 1 : j] = T[i - 1];
 }
 
 __global__ void bwt_emit_indexes(const u32 *__restrict__ rank, u32 n, u32 r, u32 count, u32 *mail)

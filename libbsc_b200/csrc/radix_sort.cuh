@@ -384,9 +384,10 @@ static inline size_t rs_scratch_bytes(u32 n, int npasses)
 
 // Sort n elements.  Pass 0 reads from `first`; later passes ping-pong between (k[0],v[0]) and
 // (k[1],v[1]), pass p writing to buffer (p & 1).  Returns the index of the buffer holding the
-// sorted result.  `scratch` must hold rs_scratch_bytes(n, passes.count).
+// sorted result.  `scratch` must hold rs_scratch_bytes(n, passes.count).  `name`: the passes' name in the profile.
 template <typename K, bool HAS_VAL, class FirstSrc>
-static int rs_sort(Ctx *ctx, FirstSrc first, K *const k[2], u32 *const v[2], u32 n, const DigitPasses &passes, void *scratch)
+static int rs_sort(Ctx *ctx, FirstSrc first, K *const k[2], u32 *const v[2], u32 n, const DigitPasses &passes, void *scratch,
+                   const char *name = "rs_onesweep")
 {
     if (passes.count == 0 || n == 0) return -1;
     const u32 tiles = ceil_div(n, RS_TILE);
@@ -417,11 +418,11 @@ static int rs_sort(Ctx *ctx, FirstSrc first, K *const k[2], u32 *const v[2], u32
         const int s2 = more ? (int)passes.shift[p + 1] : 0, b2 = more ? (int)passes.bits[p + 1] : 1;
         PROF_BYTES(ctx, pass_bytes);
         if (p == 0) {
-            LAUNCH_NAMED(ctx, "rs_onesweep", k_first, tiles, RS_THREADS, smem,
+            LAUNCH_NAMED(ctx, name, k_first, tiles, RS_THREADS, smem,
                    first, k[dst], v[dst], n, (int)passes.shift[p], (int)passes.bits[p], ghist + 256 * p, hnext, s2, b2, counters + p, lb);
         } else if (!rs_use_tma()) {
             SrcArray<K, HAS_VAL> src{k[dst ^ 1], v[dst ^ 1]};
-            LAUNCH_NAMED(ctx, "rs_onesweep", k_next, tiles, RS_THREADS, smem,
+            LAUNCH_NAMED(ctx, name, k_next, tiles, RS_THREADS, smem,
                    src, k[dst], v[dst], n, (int)passes.shift[p], (int)passes.bits[p], ghist + 256 * p, hnext, s2, b2, counters + p, lb);
         } else {
             const u32 grid = min(tiles, device_sms(ctx->device) * 2);                // persistent: two CTAs per SM, each loops over tiles
